@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- LLD frames/s of the B200 path on the BASELINE.json configurations.
+"""bench.py -- LLD frames/s of the CUDA path on the BASELINE.json configurations.
 
 A "step" is one pass of the hot path over one batch of synthetic utterances (weak scaling: every rank owns its own batch; the
 path has no data-path collective, NCCL only carries the timing / counter reduction).
@@ -32,7 +32,13 @@ path has no data-path collective, NCCL only carries the timing / counter reducti
                  (what a shell loop over files gets; dominated by process start-up and component registration).
 
 `--impl reference` times the reference's own CPU implementation as its own line (same legs).
+
+`--dump-outputs DIR` writes, after the timed steps, what the timed path (osm_b200_plan_run_device) returned in its last step:
+DIR/lld_rows.npy (float32) holds the LLD rows -- all of them when they fit in 64 MB, else a fixed, seeded sample of whole rows --
+and DIR/lld_row_index.npy (float64) their row numbers.  The synthetic batch is seeded, so two builds run with the same arguments
+can be compared output for output.
 """
+import atexit
 import argparse
 import json
 import os
@@ -109,7 +115,7 @@ def synth_batch_torch(w, device, seed):
 
 
 class ClockSampler:
-    """nvidia-smi clock / throttle sampling during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clock / throttle sampling during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -127,10 +133,16 @@ class ClockSampler:
             self.proc = subprocess.Popen(["nvidia-smi", "-i", str(self.idx), "--query-gpu=" + self.Q,
                                           "--format=csv,noheader,nounits", "-lms", "20"],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
+            atexit.register(self._kill)                 # the sampler never outlives the benchmark, even when a step fails
             self.th = threading.Thread(target=self._read, daemon=True)
             self.th.start()
         except Exception:
             self.proc = None
+
+    def _kill(self):
+        if self.proc is not None and self.proc.poll() is None:
+            self.proc.kill()
+            self.proc.wait()
 
     def _read(self):
         for ln in self.proc.stdout:
@@ -171,18 +183,7 @@ def measured_peak_hbm():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def profile_traffic():
-    """dram bytes per launch of the fused kernel from the committed ncu capture, if any."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p)).get("lld_kernel_dram_bytes_per_launch")
-        except Exception:
-            return None
-    return None
+    return 3350.0, "fallback: NVIDIA H100 SXM data sheet, 3.35 TB/s (not measured)"
 
 
 def bind_to_gpu_numa_node(local_rank):
@@ -423,7 +424,22 @@ def make_plan(w, local_rank):
     return Plan(list(comps), level, device=local_rank)
 
 
-def measure(w, args, rank, world, local_rank, dist, steps, with_cpu, sampler=None):
+DUMP_BYTES = 64 * 1000 * 1000 - 4096         # --dump-outputs: at most 64 MB in all (.npy headers included)
+
+
+def dump_outputs(dump_dir, d_out):
+    """--dump-outputs: the rows of the last timed step; a fixed, seeded sample of whole rows when all of them exceed DUMP_BYTES"""
+    import torch
+    rows, cols = d_out.shape
+    n = min(rows, DUMP_BYTES // (cols * 4 + 8))
+    idx = np.arange(rows) if n == rows else np.sort(np.random.default_rng(0).choice(rows, n, replace=False))
+    got = d_out[torch.from_numpy(idx).to(d_out.device)].cpu().numpy()
+    os.makedirs(dump_dir, exist_ok=True)
+    np.save(os.path.join(dump_dir, "lld_rows.npy"), got.astype(np.float32))
+    np.save(os.path.join(dump_dir, "lld_row_index.npy"), idx.astype(np.float64))
+
+
+def measure(w, args, rank, world, local_rank, dist, steps, with_cpu, sampler=None, dump_dir=None):
     """one workload on this rank's GPU; returns the JSON-able result dict (rank 0) or None"""
     import torch
     from opensmile_b200.dist import reduce_counters
@@ -461,6 +477,8 @@ def measure(w, args, rank, world, local_rank, dist, steps, with_cpu, sampler=Non
     ev1.record()
     barrier()
     dt_ms = ev0.elapsed_time(ev1)
+    if dump_dir is not None and rank == 0:
+        dump_outputs(dump_dir, d_out)
     # kernel times need a sync per step: taken in a separate pass so the timed loop stays free of host synchronisation
     lld_ms, post_ms = [], []
     for _ in range(min(steps, 10)):
@@ -505,7 +523,7 @@ def measure(w, args, rank, world, local_rank, dist, steps, with_cpu, sampler=Non
         if w.key == "mfcc12":
             k_ms = statistics.mean(lld_ms)
             roof = {"bound": "hbm", "achieved": alg / (k_ms * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
-                    "traffic": profile_traffic(),
+                    "traffic": None,
                     "kernel": "lld_kernel<256,32,256,2,VEC2,MFCC>" if os.environ.get("OSM_B200_LLD_FAST", "1")[:1] == "0" else "lld512_kernel<13>",
                     "kernel_ms": k_ms,
                     "post_kernel_ms": statistics.mean(post_ms), "algorithmic_bytes_per_launch": alg, "peak_source": peak_src}
@@ -522,7 +540,7 @@ def measure(w, args, rank, world, local_rank, dist, steps, with_cpu, sampler=Non
             "n_gpus": world, "steps": steps, "warmup": args.warmup, "ms_per_step": ms_step,
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": w.title, "frames_per_gpu_per_step": rows,
-                       "l2": "no flush needed: per step %d MB PCM in + %d MB rows out exceed the 126 MB L2" % (h2d // 1000000, d2h // 1000000),
+                       "l2": "no flush needed: per step %d MB PCM in + %d MB rows out exceed the 50 MB L2" % (h2d // 1000000, d2h // 1000000),
                        "parallelism": "utterance shards, one rank per GPU, no data-path collective"},
             "clocks": clocks,
             "e2e": {"value": e2e_value, "unit": "frames/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h, "steps": steps,
@@ -580,11 +598,12 @@ def run_ours(args, rank, world, local_rank):
         dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", local_rank))
     w = workload(args.workload)
     sampler = ClockSampler(local_rank) if rank == 0 else None
-    line = measure(w, args, rank, world, local_rank, dist, args.steps, with_cpu=(world == 1), sampler=sampler)
+    line = measure(w, args, rank, world, local_rank, dist, args.steps, with_cpu=(world == 1), sampler=sampler,
+                   dump_dir=args.dump_outputs)
     others = []
     if not args.no_others and args.workload == "mfcc12":
         for key in ("egemaps", "compare16", "plp44k"):
-            r = measure(workload(key), args, rank, world, local_rank, dist, max(3, min(args.steps, 5)), with_cpu=(world == 1))
+            r = measure(workload(key), args, rank, world, local_rank, dist, min(args.steps, 5), with_cpu=(world == 1))
             if r is not None:
                 others.append({k: r[k] for k in ("value", "unit", "ms_per_step", "steps", "config", "e2e", "gpu_launches", "roofline",
                                                  "parity", "cpu_baseline") if k in r})
@@ -618,6 +637,8 @@ def main():
                          "plp44k = configs[4] (44.1 kHz stereo)")
     ap.add_argument("--no-others", action="store_true", default=os.environ.get("OSM_BENCH_NO_OTHERS") == "1",
                     help="mfcc12 only: do not append the short measurements of the other three configurations")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the rows of the last step as DIR/*.npy (at most 64 MB)")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3

@@ -1,5 +1,5 @@
 /*
- * osm_b200.h -- C ABI of libosm_b200.so: the B200 (sm_100a) back end for openSMILE's
+ * osm_b200.h -- C ABI of libosm_b200.so: the H100 (sm_90a) back end for openSMILE's
  * per-frame low-level-descriptor (LLD) extraction path.
  *
  * Boundary (SURVEY.md 8b).  In the reference every LLD component is a cSmileComponent

@@ -1,4 +1,4 @@
-"""opensmile_b200 -- B200 (sm_100a) back end for openSMILE's per-frame LLD extraction path.
+"""opensmile_b200 -- H100 (sm_90a) back end for openSMILE's per-frame LLD extraction path.
 
 The compute path is the in-tree CUDA library libosm_b200.so behind the C ABI in
 include/osm_b200.h; importing this package does not load it, the first use of

@@ -1,4 +1,4 @@
-// formant.cu -- the formant chain of the GeMAPS graphs as one kernel (sm_100a):
+// formant.cu -- the formant chain of the GeMAPS graphs as one kernel (sm_90a):
 //   cWindower level -> [cTransformFFT -> cSpecResample] -> cLpc (acf) -> cFormantLpc        (SURVEY.md 8f-2)
 //
 // The reference transforms every windowed frame (zero padded to the FFT size), and cSpecResample evaluates an

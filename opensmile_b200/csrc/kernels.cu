@@ -1,4 +1,4 @@
-// kernels.cu -- fused per-frame LLD kernels for sm_100a.
+// kernels.cu -- fused per-frame LLD kernels for sm_90a.
 //
 // Design (see DESIGN.md): one persistent CTA processes "tiles" of F consecutive frames of one
 // utterance.  Inside a tile every thread keeps the mapping  lane -> frame  for ALL phases:

@@ -1,11 +1,11 @@
-// kernels.cuh -- parameter blocks and launchers of the fused LLD kernels (sm_100a).
+// kernels.cuh -- parameter blocks and launchers of the fused LLD kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
 
 // The kernels that read PCM (kernels.cu, ops.cu, pitch.cu, formant.cu) are compiled TWICE (Makefile): the default objects read
-// int16 only (OSM_PCM_F32_SUPPORT = 0) -- measured on the B200, a run-time "float samples?" test inside the sample accessors cost the
-// ComParE step 5 ms device-resident and 20 % of its end-to-end rate (profiles/r02_e2e_regression_bisect.txt) -- and the _f32 objects
+// int16 only (OSM_PCM_F32_SUPPORT = 0) -- a run-time "float samples?" test inside the sample accessors made the ComParE step
+// measurably slower, device-resident and end to end -- and the _f32 objects
 // (-DOSM_F32_VARIANT) read the mono float buffer pcm_convert_kernel produces for the other sample formats.  Under OSM_F32_VARIANT every
 // external function of those translation units gets the suffix _f32; api.cu picks launch_*_f32 for plans whose input is not int16.
 #ifdef OSM_F32_VARIANT

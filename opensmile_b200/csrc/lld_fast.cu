@@ -1,4 +1,4 @@
-// lld_fast.cu -- the 512-point mono MFCC instance of the fused per-frame kernel (sm_100a).
+// lld_fast.cu -- the 512-point mono MFCC instance of the fused per-frame kernel (sm_90a).
 //
 // Same contract, shared-memory layout, tables, chunk / tile geometry and results as lld_kernel<256,32,256,2,VEC2,MFCC>
 // (kernels.cu); launch_lld() selects it when the pass is: N = 512, one channel, cMfcc on the power spectrum, no
@@ -22,7 +22,7 @@
 
 // A/B switch: 1 = a warp adds its finished log band values straight into partial DCT sums (balanced, no band level in
 // shared memory) -- 4 % faster, but the partial sums reorder the reference's sequential m = 0..25 accumulation, which moves
-// 0.3 % of the delta-delta values past 1e-5 of their column's scale (measured, profiles/r02_v3_*).  Default: reference order.
+// 0.3 % of the delta-delta values past 1e-5 of their column's scale (measured).  Default: reference order.
 #ifndef OSM_FAST_FUSED_DCT
 #define OSM_FAST_FUSED_DCT 0
 #endif

@@ -1,4 +1,4 @@
-// pitch.cu -- the sub-harmonic-summation pitch chain of the ComParE / GeMAPS graphs (SURVEY.md 8f-1), sm_100a:
+// pitch.cu -- the sub-harmonic-summation pitch chain of the ComParE / GeMAPS graphs (SURVEY.md 8f-1), sm_90a:
 //   shs_kernel       cSpecScale + cPitchShs (+ cPitchBase output logic), one WARP per frame
 //   viterbi_kernel   cPitchSmootherViterbi [+ cValbasedSelector], one THREAD per utterance (sequential in time)
 //   jitter_kernel    cPitchJitter, one WARP per utterance (sequential over frames and pitch periods, lanes =
@@ -483,9 +483,8 @@ __global__ void __launch_bounds__(64) viterbi_kernel(const ViterbiParams p, int 
   }
 }
 
-// The same smoother with one WARP per utterance -- an A/B variant (-DOSM_VITERBI_WARP=1), NOT the default: measured on the B200
-// (ComParE workload, 10 000 utterances x 296 frames, profiles/r02_v10_viterbi_ab.txt) it takes 9.2 ms against 7.3 ms for the
-// one-thread kernel above.  A thread-per-utterance warp instruction advances 32 utterances; here it advances one, and what the lanes
+// The same smoother with one WARP per utterance -- an A/B variant (-DOSM_VITERBI_WARP=1), NOT the default: on the ComParE workload
+// (10 000 utterances x 296 frames) it was slower than the one-thread kernel above.  A thread-per-utterance warp instruction advances 32 utterances; here it advances one, and what the lanes
 // share (13 logarithms, 120 path bytes, <= 30 candidate frames) fills a fraction of them, so ~6x more instructions are issued for the
 // same work and 64 resident warps per SM do not make up for it.  What is sequential in the reference stays sequential and is executed redundantly by all lanes on shared
 // operands: the (i, j) transition walk with its running `lastChange` (hpp:224-252).  Everything around it is spread over the lanes:
@@ -710,7 +709,7 @@ __device__ void jit_extrema(const float *x, int N, int lane, float &mx, int &mI,
 
 // 5 CTAs / SM: 96 registers per thread (a few spilled words outside the loops) -> 20 warps / SM instead of 16
 #ifndef OSM_JIT_MIN_BLOCKS
-#define OSM_JIT_MIN_BLOCKS 6   // 80 registers: six CTAs (24 warps) per SM; A/B on B200 (ComParE, 10 k utterances): 55.0 -> 52.6 ms
+#define OSM_JIT_MIN_BLOCKS 6   // 80 registers: six CTAs (24 warps) per SM; faster than five on the ComParE workload (10 k utterances)
 #endif
 __global__ void __launch_bounds__(kJitWarps * 32, OSM_JIT_MIN_BLOCKS) jitter_kernel(const JitterParams p, int u0, int u1)
 {
