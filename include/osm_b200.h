@@ -45,7 +45,8 @@ extern "C" {
 #endif
 
 /* 2: component types cSpecScale .. cPitchJitter appended (existing values and struct layouts unchanged)
- * 3: cSpecResample, cLpc, cFormantLpc, cDataSelector, cHarmonics appended (same rule; sizeof(osm_b200_component) grows) */
+ * 3: cSpecResample, cLpc, cFormantLpc, cDataSelector, cHarmonics appended (same rule; sizeof(osm_b200_component) grows);
+ *    later cLsp appended under the same number: a new enum value at the end, no struct layout or size changes */
 #define OSM_B200_ABI_VERSION 3
 #if defined(__GNUC__)
 #define OSM_B200_API __attribute__((visibility("default")))
@@ -98,6 +99,7 @@ typedef enum {
   OSM_B200_C_FORMANTLPC,         /* cFormantLpc         src/lld/formantLpc.cpp:192-394 (root solving branch) */
   OSM_B200_C_DATASELECTOR,       /* cDataSelector       src/core/dataSelector.cpp:296-366 (elementMode=1)    */
   OSM_B200_C_HARMONICS,          /* cHarmonics          src/lld/harmonics.cpp:743-935 (GeMAPS switch set)    */
+  OSM_B200_C_LSP,                /* cLsp                src/lld/lsp.cpp:113-313 (on a stand-alone cLpc level) */
   OSM_B200_C_COUNT_
 } osm_b200_component_type;
 
@@ -336,6 +338,10 @@ typedef struct {            /* cHarmonics: reader.dmLevel = <pitch level>;<forma
   double  logRelValueFloorUnvoiced;                      /* -201 */
 } osm_b200_harmonics;
 
+typedef struct {            /* cLsp: reads a cLpc level (its lpcCoeff field) */
+  int32_t processArrayFields;   /* 1 (the cVectorProcessor default); only 0 is supported */
+} osm_b200_lsp;
+
 /* one `[name:cType]` section */
 typedef struct {
   int32_t type;                                  /* osm_b200_component_type */
@@ -378,6 +384,7 @@ typedef struct {
     osm_b200_formantlpc formantlpc;
     osm_b200_dataselector dataselector;
     osm_b200_harmonics harmonics;
+    osm_b200_lsp lsp;
   } u;
 } osm_b200_component;
 

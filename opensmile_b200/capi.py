@@ -22,7 +22,7 @@ OK, ERR_INVALID, ERR_UNSUPPORTED, ERR_CUDA, ERR_NOMEM = range(5)
  C_MELSPEC, C_MFCC, C_PLP, C_SPECTRAL, C_ENERGY, C_MZCR, C_ACF, C_PITCHACF,
  C_DELTAREGRESSION, C_CONTOURSMOOTHER, C_VECTORCONCAT, C_VECTOROPERATION, C_FULLINPUTMEAN, C_INTENSITY,
  C_SPECSCALE, C_PITCHSHS, C_PITCHSMOOTHERVITERBI, C_VALBASEDSELECTOR, C_PITCHJITTER,
- C_SPECRESAMPLE, C_LPC, C_FORMANTLPC, C_DATASELECTOR, C_HARMONICS) = range(30)
+ C_SPECRESAMPLE, C_LPC, C_FORMANTLPC, C_DATASELECTOR, C_HARMONICS, C_LSP) = range(31)
 
 TYPE_BY_NAME = {
     "cWaveSource": C_WAVESOURCE, "cExternalAudioSource": C_WAVESOURCE, "cFramer": C_FRAMER,
@@ -36,7 +36,7 @@ TYPE_BY_NAME = {
     "cSpecScale": C_SPECSCALE, "cPitchShs": C_PITCHSHS, "cPitchSmootherViterbi": C_PITCHSMOOTHERVITERBI,
     "cValbasedSelector": C_VALBASEDSELECTOR, "cPitchJitter": C_PITCHJITTER,
     "cSpecResample": C_SPECRESAMPLE, "cLpc": C_LPC, "cFormantLpc": C_FORMANTLPC,
-    "cDataSelector": C_DATASELECTOR, "cHarmonics": C_HARMONICS,
+    "cDataSelector": C_DATASELECTOR, "cHarmonics": C_HARMONICS, "cLsp": C_LSP,
 }
 
 WIN_BY_NAME = {"rec": 0, "han": 1, "ham": 2, "gau": 3, "sin": 4, "tri": 5, "bar": 6}
@@ -217,6 +217,10 @@ class Harmonics(C.Structure):
                 ("computeAcfHnrLogdB", i32), ("computeAcfHnrLinear", i32), ("logRelValueFloorUnvoiced", f64)]
 
 
+class Lsp(C.Structure):
+    _fields_ = [("processArrayFields", i32)]
+
+
 class _U(C.Union):
     _fields_ = [("wavesource", WaveSource), ("framer", Framer),
                 ("vectorpreemphasis", VectorPreemphasis), ("windower", Windower),
@@ -228,7 +232,7 @@ class _U(C.Union):
                 ("specscale", SpecScale), ("pitchshs", PitchShs), ("pitchsmootherviterbi", PitchSmootherViterbi),
                 ("valbasedselector", ValbasedSelector), ("pitchjitter", PitchJitter),
                 ("specresample", SpecResample), ("lpc", Lpc), ("formantlpc", FormantLpc),
-                ("dataselector", DataSelector), ("harmonics", Harmonics)]
+                ("dataselector", DataSelector), ("harmonics", Harmonics), ("lsp", Lsp)]
 
 
 class Component(C.Structure):
@@ -344,6 +348,8 @@ def lib():
     if L.osm_b200_sizeof_component() != C.sizeof(Component):
         raise RuntimeError("ABI mismatch: sizeof(osm_b200_component) = %d, ctypes mirror = %d"
                            % (L.osm_b200_sizeof_component(), C.sizeof(Component)))
+    if L.osm_b200_component_defaults(C_LSP, C.byref(Component())) != 0:     # the last component type of this mirror
+        raise RuntimeError("ABI mismatch: the library does not know component type %d (cLsp)" % C_LSP)
     _lib = L
     return L
 

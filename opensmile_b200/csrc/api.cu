@@ -23,6 +23,8 @@ cudaError_t launch_energy_f32(const TimeOpParams &p, cudaStream_t st);
 cudaError_t launch_mzcr_f32(const TimeOpParams &p, cudaStream_t st);
 cudaError_t launch_intensity_f32(const TimeOpParams &p, cudaStream_t st);
 cudaError_t launch_formant_f32(const FormantParams &p, cudaStream_t st);
+cudaError_t launch_lpc_f32(const LpcParams &p, cudaStream_t st);
+size_t lpc_smem_bytes_f32(const LpcParams &p);
 cudaError_t launch_jitter_f32(const JitterParams &p, int u0, int u1, cudaStream_t st);
 }
 
@@ -192,6 +194,7 @@ struct OpRt {
   HarmonicsParams hrm;                  // SOP_HARMONICS
   double *dCosTab = nullptr;            // its cos(2 pi m / N) table
   FormantParams fmt;                    // SOP_FORMANT
+  LpcParams lpc;                        // SOP_LPC
   float *dFmtD = nullptr;               // its resampling table
   unsigned char *dPitchTab = nullptr;   // spline / interpolation / harmonic tables of the chain
   DevBuf<float> dShs;                   // [static rows][nShsCols] cPitchShs level
@@ -345,6 +348,7 @@ osm_b200_status osm_b200_component_defaults(int32_t type, osm_b200_component *c)
     }
     case OSM_B200_C_SPECRESAMPLE: c->u.specresample.targetFs = 16000.0; c->u.specresample.resampleRatio = -1.0; break;   // dsp/specResample.cpp:40-41
     case OSM_B200_C_LPC: c->u.lpc.p = 8; c->u.lpc.saveLPCoeff = 1; break;                                               // lld/lpc.cpp:33-45
+    case OSM_B200_C_LSP: c->u.lsp.processArrayFields = 1; break;                                                       // core/vectorProcessor.cpp:37
     case OSM_B200_C_DATASELECTOR: c->u.dataselector.elementMode = 1; break;                                              // core/dataSelector.cpp:39
     case OSM_B200_C_HARMONICS: {           // lld/harmonics.cpp:28-56
       auto &q = c->u.harmonics;
@@ -869,6 +873,7 @@ osm_b200_status osm_b200_plan_create(const osm_b200_component *comps, int32_t n_
       ap.F = srt.tileF;     // width of the magnitude level's tiles
       ap.nfft = fe.nfft; ap.nSrc = fe.nBins;
       ap.acfUsePower = po.acfUsePower; ap.cepUsePower = po.cepUsePower; ap.absCepstrum = po.absCepstrum; ap.normOutput = po.normOutput;
+      ap.oldCompatCepstrum = po.oldCompatCepstrum;
       ap.maxPitch = po.maxPitch; ap.voicingCutoff = po.voicingCutoff; ap.fsSec = po.fsSec;
       ap.voiceProb = po.voiceProb; ap.voiceQual = po.voiceQual; ap.HNR = po.HNR; ap.HNRdB = po.HNRdB; ap.linHNR = po.linHNR;
       ap.F0 = po.F0; ap.F0raw = po.F0raw; ap.F0env = po.F0env;
@@ -901,6 +906,12 @@ osm_b200_status osm_b200_plan_create(const osm_b200_component *comps, int32_t n_
         fp.refOrder = fo.refOrder ? 1 : 0; fp.kHalf = fo.kHalf; fp.padLeft = fo.padLeft; fp.halfK = fo.halfK;
         fp.saveFormants = fo.saveFormants; fp.saveBandwidths = fo.saveBandwidths; fp.saveNValid = fo.saveNValid;
         if (formant_smem_bytes(fp) > 200 * 1024) { pl->ops.push_back(rt); osm_b200_plan_destroy(pl); return fail(OSM_B200_ERR_UNSUPPORTED, "cSpecResample: frame too long for the formant kernel"); }
+      } else if (op.kind == SOP_LPC) {
+        LpcParams &lp = rt.lpc;
+        memset(&lp, 0, sizeof lp);
+        tp.preemph = fe.preemph;                   // the level cLpc reads: pre-emphasised whenever its chain has the stage
+        lp.tp = tp; lp.p = op.lpc.p; lp.outLpc = op.lpc.lpc; lp.outGain = op.lpc.gain; lp.outLsp = op.lpc.lsp;
+        if (lpc_smem_bytes(lp) > 200 * 1024) { osm_b200_plan_destroy(pl); return fail(OSM_B200_ERR_UNSUPPORTED, "cLpc: frame too long for the LPC kernel"); }
       } else if (op.kind == SOP_ENERGY) {
         const EnergyOp &e = op.energy;
         tp.eHtk = e.htk; tp.eRms = e.rms; tp.eEnergy2 = e.energy2; tp.eLog = e.lg;
@@ -1263,6 +1274,7 @@ static osm_b200_status launch_range(osm_b200_plan *pl, const void *d_pcm, float 
       tp.tiles = rt.dTiles.p + t0; tp.nTiles = t1 - t0;
       tp.stat = pl->dStat.p;
       if (o.kind == SOP_FORMANT) { FormantParams fp = o.fmt; fp.tp = tp; CU((f32in ? launch_formant_f32 : launch_formant)(fp, st)); PROF("formant_kernel"); }
+      else if (o.kind == SOP_LPC) { LpcParams lp = o.lpc; lp.tp = tp; CU((f32in ? launch_lpc_f32 : launch_lpc)(lp, st)); PROF("lpc_kernel"); }
       else {
         CU(o.kind == SOP_ENERGY ? (f32in ? launch_energy_f32 : launch_energy)(tp, st)
                                 : (o.kind == SOP_INTENSITY ? (f32in ? launch_intensity_f32 : launch_intensity)(tp, st) : (f32in ? launch_mzcr_f32 : launch_mzcr)(tp, st)));

@@ -35,7 +35,7 @@ const char *type_name(int t)
     "cTransformFFT", "cFFTmagphase", "cMelspec", "cMfcc", "cPlp", "cSpectral", "cEnergy",
     "cMZcr", "cAcf", "cPitchACF", "cDeltaRegression", "cContourSmoother", "cVectorConcat",
     "cVectorOperation", "cFullinputMean", "cIntensity", "cSpecScale", "cPitchShs", "cPitchSmootherViterbi",
-    "cValbasedSelector", "cPitchJitter", "cSpecResample", "cLpc", "cFormantLpc", "cDataSelector", "cHarmonics"};
+    "cValbasedSelector", "cPitchJitter", "cSpecResample", "cLpc", "cFormantLpc", "cDataSelector", "cHarmonics", "cLsp"};
   return (t >= 0 && t < OSM_B200_C_COUNT_) ? names[t] : "?";
 }
 
@@ -471,8 +471,9 @@ osm_b200_status compile_graph(const osm_b200_component *comps, int n, const char
         if (a->u.acf.cepstrum || !b->u.acf.cepstrum) { err = "cPitchACF expects [acf ; cepstrum] in this order"; return OSM_B200_ERR_UNSUPPORTED; }
         for (const osm_b200_component *x : {a, b}) {
           const auto &q = x->u.acf;
-          if (q.inverse || q.cosLifterCepstrum || q.oldCompatCepstrum || !q.symmetricData) { err = "cAcf: inverse / cosLifterCepstrum / oldCompatCepstrum / symmetricData=0 are not supported"; return OSM_B200_ERR_UNSUPPORTED; }
+          if (q.inverse || q.cosLifterCepstrum || !q.symmetricData) { err = "cAcf: inverse / cosLifterCepstrum / symmetricData=0 are not supported"; return OSM_B200_ERR_UNSUPPORTED; }
         }
+        // oldCompatCepstrum only changes the cepstrum's input stage; on the ACF instance it has no effect (dspcore/acf.cpp:103-109,276)
         if (single_input(a) != single_input(b)) { err = "both cAcf instances must read the same cFFTmagphase level"; return OSM_B200_ERR_UNSUPPORTED; }
         if (!resolve_mag_chain(single_input(a), ci)) return OSM_B200_ERR_UNSUPPORTED;
         osm_b200_status s2 = get_stream(ci, true, op.stream);
@@ -481,9 +482,11 @@ osm_b200_status compile_graph(const osm_b200_component *comps, int n, const char
         op.kind = SOP_PITCHACF;
         PitchAcfOp &po = op.pitch;
         po.acfUsePower = a->u.acf.usePower != 0; po.cepUsePower = b->u.acf.usePower != 0;
-        po.absCepstrum = b->u.acf.absCepstrum != 0;
+        po.oldCompatCepstrum = b->u.acf.oldCompatCepstrum != 0;
+        po.absCepstrum = b->u.acf.absCepstrum != 0 || po.oldCompatCepstrum;                  // oldCompatCepstrum forces absCepstrum = 1
         po.normOutput = a->u.acf.acfCepsNormOutput != 0;
-        if ((b->u.acf.acfCepsNormOutput != 0) != po.normOutput) { err = "cAcf.acfCepsNormOutput must agree on both instances"; return OSM_B200_ERR_UNSUPPORTED; }
+        const bool cepNorm = b->u.acf.acfCepsNormOutput != 0 && !po.oldCompatCepstrum;     // ... and acfCepsNormOutput = 0
+        if (cepNorm != po.normOutput) { err = "cAcf.acfCepsNormOutput must agree on both instances"; return OSM_B200_ERR_UNSUPPORTED; }
         const auto &pp = c->u.pitchacf;
         po.maxPitch = pp.maxPitch < 0.0 ? 0.0 : pp.maxPitch;                       // lldcore/pitchACF.cpp:101-102
         po.voicingCutoff = pp.voicingCutoff > 1.0 ? 1.0 : (pp.voicingCutoff < 0.0 ? 0.0 : pp.voicingCutoff);
@@ -606,6 +609,46 @@ osm_b200_status compile_graph(const osm_b200_component *comps, int n, const char
         if (op.formant.saveNValid) { FieldName f; f.name = "nFormants"; op.fields.push_back(f); }
         if (op.formant.saveFormants) { FieldName f; f.name = "formantFreqLpc"; f.n = op.formant.nFormants; f.arrNameOffset = 1; op.fields.push_back(f); }
         if (op.formant.saveBandwidths) { FieldName f; f.name = "formantBandwidthLpc"; f.n = op.formant.nFormants; f.arrNameOffset = 1; op.fields.push_back(f); }
+      } else if (c->type == OSM_B200_C_LPC || c->type == OSM_B200_C_LSP) {
+        // stand-alone cLpc (method acf) on a time-domain frame level [framer -> pre-emphasis -> window], and cLsp on such a
+        // cLpc level (config/emobase/emobase.conf: cVectorPreemphasis -> cLpc p = 8 -> cLsp).  Both are cVectorProcessors
+        // that keep the frame count of the level they read.
+        const osm_b200_component *lpc = c;
+        if (c->type == OSM_B200_C_LSP) {
+          if (c->u.lsp.processArrayFields != 0) { err = "cLsp.processArrayFields=1 is not supported (the reference's cLsp finds its input field only with processArrayFields=0)"; return OSM_B200_ERR_UNSUPPORTED; }
+          lpc = single_input(c);
+          if (!lpc || lpc->type != OSM_B200_C_LPC || !lpc->u.lpc.saveLPCoeff) { err = "cLsp must read a level with an lpcCoeff field (a cLpc level with saveLPCoeff=1)"; return OSM_B200_ERR_UNSUPPORTED; }
+          // lld/lsp.cpp:289-292: with more input elements than lspFreq outputs (Ndst < Nsrc) the reference's cLsp writes nothing
+          if (lpc->u.lpc.lpGain) { err = "cLsp reading a cLpc level that also holds lpGain is not supported (Ndst < Nsrc: the reference's cLsp returns without output, lld/lsp.cpp:292)"; return OSM_B200_ERR_UNSUPPORTED; }
+        }
+        const auto &q = lpc->u.lpc;
+        if (q.method != 0) { err = "cLpc: only method=acf is supported (burg is not)"; return OSM_B200_ERR_UNSUPPORTED; }
+        if (q.saveRefCoeff || q.residual || q.forwardFilter || q.lpSpectrum) { err = "cLpc: saveRefCoeff / residual / forwardFilter / lpSpectrum are not supported"; return OSM_B200_ERR_UNSUPPORTED; }
+        if (q.p < 1 || q.p > 16) { err = "cLpc.p must be in 1..16"; return OSM_B200_ERR_UNSUPPORTED; }
+        if (!q.saveLPCoeff && !q.lpGain) { err = "cLpc produces no output"; return OSM_B200_ERR_INVALID; }
+        const osm_b200_component *in = single_input(lpc);
+        if (in && in->type == OSM_B200_C_SPECRESAMPLE) {
+          err = c->type == OSM_B200_C_LSP ? "cLsp behind the formant chain's cSpecResample -> cLpc is not supported"
+                                          : "cLpc on a cSpecResample level is supported only in front of cFormantLpc";
+          return OSM_B200_ERR_UNSUPPORTED;
+        }
+        if (!resolve_time_chain(in, ci)) { err = "cLpc: " + err; return OSM_B200_ERR_UNSUPPORTED; }
+        op.windowed = ci.win != nullptr;
+        osm_b200_status s2 = get_stream(ci, false, op.stream);
+        if (s2 != OSM_B200_OK) return s2;
+        op.kind = SOP_LPC;
+        op.lpc.p = q.p;
+        FieldName f;
+        if (c->type == OSM_B200_C_LSP) {                                     // lld/lsp.cpp:272-287
+          op.lpc.lpc = false; op.lpc.lsp = true;
+          f.name = "lspFreq"; f.n = q.p; op.fields.push_back(f);
+        } else {                                                             // lld/lpc.cpp:118-146
+          op.lpc.lpc = q.saveLPCoeff != 0; op.lpc.gain = q.lpGain != 0;
+          if (op.lpc.lpc) { f.name = "lpcCoeff"; f.n = q.p; op.fields.push_back(f); }
+          if (op.lpc.gain) { FieldName g; g.name = "lpGain"; op.fields.push_back(g); }
+        }
+        op.nOut = 0;
+        for (const FieldName &x : op.fields) op.nOut += x.n;
       } else if (c->type == OSM_B200_C_HARMONICS) {
         // cHarmonics reads [pitch level ; formant level ; magnitude level] through one multi-level reader
         // (GeMAPSv01b_core.lld.conf.inc:289-318) and looks its inputs up by name (lld/harmonics.cpp:258-300)

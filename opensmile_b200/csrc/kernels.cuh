@@ -36,6 +36,8 @@
 #define launch_seq_post launch_seq_post_f32
 #define formant_smem_bytes formant_smem_bytes_f32
 #define launch_formant launch_formant_f32
+#define lpc_smem_bytes lpc_smem_bytes_f32
+#define launch_lpc launch_lpc_f32
 // kernels with external / weak linkage in kernels.cu and ops.cu (the other files keep theirs in anonymous namespaces)
 #define lld_kernel lld_kernel_f32
 #define acf_pitch_kernel acf_pitch_kernel_f32
@@ -226,6 +228,7 @@ struct AcfPitchParams {
   PitchRaw *raw;                 // [static rows]
   const float2 *twiddles; int twOff[4]; int twCount;
   int acfUsePower, cepUsePower, absCepstrum, normOutput;
+  int oldCompatCepstrum;         // cepstrum input: log(x) without +1, DC and Nyquist un-logged (dspcore/acf.cpp:276-286)
   double maxPitch, voicingCutoff;
   float fsSec;
   int voiceProb, voiceQual, HNR, HNRdB, linHNR, F0, F0raw, F0env;
@@ -284,6 +287,18 @@ struct FormantParams {
 };
 cudaError_t launch_formant(const FormantParams &p, cudaStream_t st);
 size_t formant_smem_bytes(const FormantParams &p);
+
+// ------------------------------------------------------------------------------------------
+// stand-alone cLpc (method acf) [-> cLsp] on a time-domain frame level (lsp.cu): one CTA per tile, one warp per frame for
+// the autocorrelation (lane = lag), then one lane per frame for Levinson-Durbin and the LSP root search
+// ------------------------------------------------------------------------------------------
+struct LpcParams {
+  TimeOpParams tp;               // frame geometry, tiles, static rows; windowed / preemph describe the level cLpc reads
+  int p;                         // predictor order
+  int outLpc, outGain, outLsp;   // columns written: lpcCoeff[p] | lpGain  (a cLpc level)  or  lspFreq[p]  (a cLsp level)
+};
+cudaError_t launch_lpc(const LpcParams &p, cudaStream_t st);
+size_t lpc_smem_bytes(const LpcParams &p);
 
 // cHarmonics (harmonics.cu): one warp per frame on the magnitude level + F0 / formant columns of the static rows
 struct HarmonicsParams {

@@ -43,7 +43,7 @@ struct FrontEnd {
   bool zeroPadSymmetric = false;   // phase only; magnitude consumers are unaffected
 };
 
-enum StaticOpKind { SOP_MFCC = 0, SOP_PLP, SOP_MELSPEC, SOP_SPECTRAL, SOP_ENERGY, SOP_MZCR, SOP_PITCHACF, SOP_VECOP, SOP_MAG, SOP_INTENSITY, SOP_PITCH, SOP_JITTER, SOP_FORMANT, SOP_HARMONICS };
+enum StaticOpKind { SOP_MFCC = 0, SOP_PLP, SOP_MELSPEC, SOP_SPECTRAL, SOP_ENERGY, SOP_MZCR, SOP_PITCHACF, SOP_VECOP, SOP_MAG, SOP_INTENSITY, SOP_PITCH, SOP_JITTER, SOP_FORMANT, SOP_HARMONICS, SOP_LPC };
 
 struct MfccOp {
   int melIdx = 0;
@@ -98,6 +98,7 @@ struct EnergyOp {
 // cAcf (ACF) + cAcf (cepstrum) -> cPitchACF (dspcore/acf.cpp, lldcore/pitchACF.cpp)
 struct PitchAcfOp {
   bool acfUsePower = true, cepUsePower = false, absCepstrum = false, normOutput = true;
+  bool oldCompatCepstrum = false;  // cepstrum of log(x) (no +1) with DC / Nyquist un-logged (dspcore/acf.cpp:103-109,276-286)
   double maxPitch = 500, voicingCutoff = 0.55;
   float fsSec = 0.f;
   bool voiceProb = true, voiceQual = false, HNR = false, HNRdB = false, linHNR = false, F0 = false, F0raw = false, F0env = false;
@@ -188,6 +189,9 @@ struct HarmonicsOp {
   int nOut = 0;
 };
 
+// stand-alone cLpc (method acf) on a time-domain frame level, or cLsp on such a cLpc level (lld/lpc.cpp, lld/lsp.cpp)
+struct LpcOp { int p = 8; bool lpc = true, gain = false, lsp = false; };
+
 // one field of a level: `n` elements named name (n == 1) or name[i + arrNameOffset]
 struct FieldName { std::string name; int n = 1; int arrNameOffset = 0; };
 
@@ -211,6 +215,7 @@ struct StaticOp {
   JitterOp jitter;
   FormantOp formant;
   HarmonicsOp harmonics;
+  LpcOp lpc;
 };
 
 // temporal stage applied to a static column range (cWindowProcessor family)

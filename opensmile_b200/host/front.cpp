@@ -236,7 +236,7 @@ const TypeInfo kTypes[] = {
   {"cPitchSmootherViterbi", OSM_B200_C_PITCHSMOOTHERVITERBI}, {"cValbasedSelector", OSM_B200_C_VALBASEDSELECTOR},
   {"cPitchJitter", OSM_B200_C_PITCHJITTER}, {"cSpecResample", OSM_B200_C_SPECRESAMPLE}, {"cLpc", OSM_B200_C_LPC},
   {"cFormantLpc", OSM_B200_C_FORMANTLPC}, {"cDataSelector", OSM_B200_C_DATASELECTOR},
-  {"cHarmonics", OSM_B200_C_HARMONICS}};
+  {"cHarmonics", OSM_B200_C_HARMONICS}, {"cLsp", OSM_B200_C_LSP}};
 
 int type_of(const std::string &t)
 {
@@ -279,6 +279,7 @@ bool to_component(const Section &s, osm_b200_component &c, std::string &err)
       SETI("includeSingleElementFields", c.u.vectorconcat.includeSingleElementFields)
       if (f == "preserveFieldNames") { if (!inum(v)) { err = "cVectorConcat.preserveFieldNames=0 is not supported"; return false; } continue; }
     }
+    if (t == OSM_B200_C_LSP && f == "processArrayFields") { c.u.lsp.processArrayFields = inum(v); continue; }
     if (is_common(f)) continue;
     switch (t) {
       case OSM_B200_C_WAVESOURCE:
