@@ -23,10 +23,12 @@
 #include <math.h>
 #include <string.h>
 
+#include <memory>
 #include <string>
 #include <vector>
 
 #include "../../include/osm_b200_functionals.h"
+#include "cuda_owned.hpp"
 #include "functionals_seq.cuh"
 #include "plan.hpp"
 
@@ -503,15 +505,14 @@ struct osm_b200_functionals {
   double period = 0;
   std::vector<std::string> names;
   bool hasPct = false, hasSeq = false, hasPeaks = false, hasSeg = false;
-  long long *dMeta = nullptr; size_t metaCap = 0;
-  float *dIn = nullptr; size_t inCap = 0;
-  float *dOut = nullptr; size_t outCap = 0;
-  int *dCols = nullptr; std::vector<int> hCols;
+  DevBuf<long long> dMeta;
+  DevBuf<float> dIn, dOut;                     // run_host staging: one float more than the largest batch so far
+  DevBuf<int> dCols; std::vector<int> hCols;
+
+  ~osm_b200_functionals() { if (device >= 0) cudaSetDevice(device); }
 };
 
 namespace {
-
-#define FCU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { char b_[256]; snprintf(b_, sizeof b_, "CUDA error in %s: %s", #call, cudaGetErrorString(e_)); return set_last_error(OSM_B200_ERR_CUDA, b_); } } while (0)
 
 std::vector<std::string> value_names(const osm_b200_functionals_spec &s)
 {
@@ -661,9 +662,10 @@ void osm_b200_functionals_defaults(osm_b200_functionals_spec *s)
   s->dct.firstCoeff = 1; s->dct.lastCoeff = 6;                    // functionalDCT.cpp:38-40
 }
 
+// no exception crosses the C boundary (host allocation failures while the names are built)
 osm_b200_status osm_b200_functionals_create(const osm_b200_functionals_spec *spec, int32_t n_in, const char *const *in_names,
                                             double input_period, int32_t device, osm_b200_functionals **out)
-{
+try {
   if (!spec || !out || n_in <= 0 || !in_names) return set_last_error(OSM_B200_ERR_INVALID, "null argument");
   *out = nullptr;
   const auto &s = *spec;
@@ -691,11 +693,11 @@ osm_b200_status osm_b200_functionals_create(const osm_b200_functionals_spec *spe
       if (G.n_thresholds < 0 || G.n_thresholds > OSM_B200_F_MAX_THRESH) return set_last_error(OSM_B200_ERR_UNSUPPORTED, "cFunctionalSegments: at most 8 thresholds");
     }
   }
-  osm_b200_functionals *f = new osm_b200_functionals();
-  f->spec = s; f->nIn = n_in; f->device = device; f->period = input_period;
+  auto f = std::make_unique<osm_b200_functionals>();
+  f->spec = s; f->nIn = n_in; f->period = input_period;
   const std::vector<std::string> vn = value_names(s);
   f->nVals = (int)vn.size();
-  if (f->nVals == 0) { delete f; return set_last_error(OSM_B200_ERR_INVALID, "cFunctionals: no value enabled"); }
+  if (f->nVals == 0) return set_last_error(OSM_B200_ERR_INVALID, "cFunctionals: no value enabled");
   for (int e = 0; e < n_in; e++)
     for (const std::string &v : vn)                                    // functionals.cpp:222-228
       f->names.push_back(s.functNameAppend[0] ? std::string(in_names[e]) + "__" + s.functNameAppend + "_" + v : std::string(in_names[e]) + "_" + v);
@@ -707,16 +709,17 @@ osm_b200_status osm_b200_functionals_create(const osm_b200_functionals_spec *spe
   }
   if (device >= 0) {
     int n = 0;
-    if (cudaGetDeviceCount(&n) != cudaSuccess || device >= n) { delete f; return set_last_error(OSM_B200_ERR_CUDA, "no usable CUDA device (this library has no CPU fallback)"); }
+    if (cudaGetDeviceCount(&n) != cudaSuccess || device >= n) return set_last_error(OSM_B200_ERR_CUDA, "no usable CUDA device (this library has no CPU fallback)");
   }
-  *out = f;
+  f->device = device;
+  *out = f.release();
   return OSM_B200_OK;
-}
+} catch (const std::bad_alloc &) { return set_last_error(OSM_B200_ERR_NOMEM, "out of host memory"); }
+catch (const std::exception &e) { return set_last_error(OSM_B200_ERR_INVALID, e.what()); }
 
 void osm_b200_functionals_destroy(osm_b200_functionals *f)
 {
   if (!f) return;
-  if (f->device >= 0) { cudaSetDevice(f->device); if (f->dMeta) cudaFree(f->dMeta); if (f->dIn) cudaFree(f->dIn); if (f->dOut) cudaFree(f->dOut); if (f->dCols) cudaFree(f->dCols); }
   delete f;
 }
 
@@ -743,13 +746,13 @@ osm_b200_status osm_b200_functionals_run_device_cols(osm_b200_functionals *f, co
   if (n_utt == 0) return OSM_B200_OK;
   if (!d_rows || !d_out || (!cols && row_stride < f->nIn) || out_stride < (int64_t)f->nVals * f->nIn) return set_last_error(OSM_B200_ERR_INVALID, "bad row buffer");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FCU(cudaSetDevice(f->device));
+  CU(cudaSetDevice(f->device));
   if (cols) {
     for (int e = 0; e < f->nIn; e++) if (cols[e] < 0 || cols[e] >= row_stride) return set_last_error(OSM_B200_ERR_INVALID, "column index outside the row");
-    if (!f->dCols || f->hCols.size() != (size_t)f->nIn || memcmp(f->hCols.data(), cols, sizeof(int) * f->nIn) != 0) {
-      if (!f->dCols) FCU(cudaMalloc(&f->dCols, sizeof(int) * (size_t)f->nIn));
+    if (!f->dCols.p || f->hCols.size() != (size_t)f->nIn || memcmp(f->hCols.data(), cols, sizeof(int) * f->nIn) != 0) {
+      CU(f->dCols.reserve_exact((size_t)f->nIn));
       f->hCols.assign(cols, cols + f->nIn);
-      FCU(cudaMemcpy(f->dCols, f->hCols.data(), sizeof(int) * (size_t)f->nIn, cudaMemcpyHostToDevice));
+      CU(cudaMemcpy(f->dCols.p, f->hCols.data(), sizeof(int) * (size_t)f->nIn, cudaMemcpyHostToDevice));
     }
   }
   long long maxT = 0;
@@ -772,18 +775,13 @@ osm_b200_status osm_b200_functionals_run_device_cols(osm_b200_functionals *f, co
   int nWarps = kFnWarps;
   while (nWarps > 1 && (size_t)nWarps * perWarp * sizeof(float) > 200 * 1024) nWarps--;
   if ((size_t)nWarps * perWarp * sizeof(float) > 200 * 1024) return set_last_error(OSM_B200_ERR_UNSUPPORTED, "cFunctionals: contour too long for the shared-memory work space");
-  if (f->metaCap < meta.size()) {
-    if (f->dMeta) cudaFree(f->dMeta);
-    f->dMeta = nullptr; f->metaCap = 0;
-    FCU(cudaMalloc(&f->dMeta, meta.size() * sizeof(long long)));
-    f->metaCap = meta.size();
-  }
-  FCU(cudaMemcpyAsync(f->dMeta, meta.data(), meta.size() * sizeof(long long), cudaMemcpyHostToDevice, st));
-  FCU(cudaStreamSynchronize(st));                  // `meta` is a local: the copy must have left the host buffer
+  CU(f->dMeta.reserve_exact(meta.size()));
+  CU(cudaMemcpyAsync(f->dMeta.p, meta.data(), meta.size() * sizeof(long long), cudaMemcpyHostToDevice, st));
+  CU(cudaStreamSynchronize(st));                  // `meta` is a local: the copy must have left the host buffer
   FnParams p;
   memset(&p, 0, sizeof p);
-  p.cols = cols ? f->dCols : nullptr; p.outStride = out_stride;
-  p.rows = d_rows; p.rowStride = row_stride; p.nIn = f->nIn; p.rowOff = f->dMeta; p.nRows = f->dMeta + n_utt;
+  p.cols = cols ? f->dCols.p : nullptr; p.outStride = out_stride;
+  p.rows = d_rows; p.rowStride = row_stride; p.nIn = f->nIn; p.rowOff = f->dMeta.p; p.nRows = f->dMeta.p + n_utt;
   p.perWarp = perWarp; p.listOff = sortCap; p.lensOff = sortCap + listFloats;
   for (int i = 0, o = 0; i < f->spec.n_enabled; i++) { p.valOff[i] = o; o += value_count(f->spec, i); }
   p.timesNorm = resolve_norm(f->spec.times.norm, f->spec.times.normIsSet, f->spec.masterTimeNorm);
@@ -798,10 +796,10 @@ osm_b200_status osm_b200_functionals_run_device_cols(osm_b200_functionals *f, co
   for (int i = 0; i < f->spec.n_enabled; i++) p.needReg = p.needReg || f->spec.enabled[i] == OSM_B200_F_REGRESSION;
   p.enQreg = R.qregc1 || R.qregc2 || R.qregc3 || R.qregerrA || R.qregerrQ || R.centroid;     // functionalRegression.cpp:108-117
   const size_t smem = (size_t)nWarps * perWarp * sizeof(float);
-  if (smem > 48 * 1024) FCU(cudaFuncSetAttribute(functionals_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (smem > 48 * 1024) CU(cudaFuncSetAttribute(functionals_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int groups = (f->nIn + nWarps - 1) / nWarps;
   functionals_kernel<<<(unsigned)((long long)n_utt * groups), nWarps * 32, smem, st>>>(p);
-  FCU(cudaGetLastError());
+  CU(cudaGetLastError());
   return OSM_B200_OK;
 }
 
@@ -832,14 +830,14 @@ osm_b200_status osm_b200_functionals_run_host(osm_b200_functionals *f, const flo
 {
   if (!f || !rows || !out || total_rows < 0) return set_last_error(OSM_B200_ERR_INVALID, "null argument");
   if (f->device < 0) return set_last_error(OSM_B200_ERR_CUDA, "description-only functionals object (device < 0) cannot run; no CPU fallback");
-  FCU(cudaSetDevice(f->device));
+  CU(cudaSetDevice(f->device));
   const size_t nIn = (size_t)total_rows * row_stride, nOut = (size_t)n_utt * f->nVals * f->nIn;
-  if (f->inCap < nIn) { if (f->dIn) cudaFree(f->dIn); f->dIn = nullptr; f->inCap = 0; FCU(cudaMalloc(&f->dIn, (nIn + 1) * sizeof(float))); f->inCap = nIn; }
-  if (f->outCap < nOut) { if (f->dOut) cudaFree(f->dOut); f->dOut = nullptr; f->outCap = 0; FCU(cudaMalloc(&f->dOut, (nOut + 1) * sizeof(float))); f->outCap = nOut; }
-  FCU(cudaMemcpy(f->dIn, rows, nIn * sizeof(float), cudaMemcpyHostToDevice));
-  osm_b200_status st = osm_b200_functionals_run_device(f, f->dIn, row_stride, row_offsets, n_rows, n_utt, f->dOut, nullptr);
+  CU(f->dIn.reserve_exact(nIn + 1));
+  CU(f->dOut.reserve_exact(nOut + 1));
+  CU(cudaMemcpy(f->dIn.p, rows, nIn * sizeof(float), cudaMemcpyHostToDevice));
+  osm_b200_status st = osm_b200_functionals_run_device(f, f->dIn.p, row_stride, row_offsets, n_rows, n_utt, f->dOut.p, nullptr);
   if (st != OSM_B200_OK) return st;
-  FCU(cudaMemcpy(out, f->dOut, nOut * sizeof(float), cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(out, f->dOut.p, nOut * sizeof(float), cudaMemcpyDeviceToHost));
   return OSM_B200_OK;
 }
 

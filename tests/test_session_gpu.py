@@ -6,6 +6,7 @@ Tolerance: float32 path, |got - ref| <= 1e-5 * (largest magnitude of that elemen
 utterance) per element -- BASELINE's 1e-5 relative bound taken per output column, because one row
 mixes quantities of very different scale (spectral variance ~1e6 Hz^2 next to a zero-crossing rate)."""
 import os
+import shutil
 import struct
 import subprocess
 import wave
@@ -15,6 +16,7 @@ import pytest
 
 from conftest import ROOT
 from opensmile_b200 import Session, pack_utterances
+from opensmile_b200.session import SessionError
 from opensmile_b200.synth import voiced_pcm
 
 pytestmark = pytest.mark.gpu
@@ -199,6 +201,27 @@ def test_mfcc_and_plp_0_d_a_confs_match_reference_goldens():
     ref = g["example_lld"]
     assert rows.shape == ref.shape == (202, 18)
     assert (np.abs(rows - ref) / np.abs(ref).max(axis=1, keepdims=True)).max() < 1e-5
+
+
+def test_device_plan_refusal_after_stream_tables_leaves_the_process_usable(tmp_path):
+    """deltawin = 7 on both delta stages sums to a half window of 14 frames: the graph opens, but building the device plan
+    refuses it after the per-stream constant tables are on the device.  The refusal carries the plan's message, and a
+    plan for the unmodified configuration still runs in the same process."""
+    src = os.path.join(CONF, "mfcc_0_d_a.conf")
+    text = open(src).read()
+    assert text.count("deltawin = 2") == 2
+    shutil.copytree(os.path.join(CONF, "inc"), tmp_path / "inc")      # the configuration's \{inc/...} include
+    wide = tmp_path / "mfcc_0_d_a_win7.conf"
+    wide.write_text(text.replace("deltawin = 2", "deltawin = 7"))
+    ex = np.load(os.path.join(ROOT, "tests", "golden", "mfcc_example_44k1.npz"))
+    pcm, sr = ex["pcm"], int(ex["sample_rate"])
+    s = Session(str(wide))
+    with pytest.raises(SessionError) as e:
+        s.extract_pcm(pcm, [0, len(pcm)], sr, 1)
+    assert str(e.value) == "summed temporal half windows exceed 12 frames"
+    s.close()
+    rows, _ = Session(src).extract_pcm(pcm, [0, len(pcm)], sr, 1)
+    assert rows.shape == (202, 39) and np.isfinite(rows).all()
 
 
 def test_cepstral_mean_subtraction_confs():
