@@ -497,6 +497,13 @@ OSM_B200_API void            osm_b200_plan_set_profiling(osm_b200_plan *plan, in
 OSM_B200_API int32_t         osm_b200_plan_profile_count(osm_b200_plan *plan);
 OSM_B200_API osm_b200_status osm_b200_plan_profile_entry(osm_b200_plan *plan, int32_t idx, const char **name, float *ms);
 
+/* The last per-frame (LLD) kernel launch of the last run_* call: *kernel = static name of the instance, e.g.
+ * "lld512_kernel<13>" or "lld_kernel<1024,8,256,1,VEC2,GEN>" (NULL when the run launched none), *grid = CTAs,
+ * *n_chunks = chunks (work units) of that launch.  run_host may launch once per pipeline piece: the last piece counts.
+ * Any pointer may be NULL. */
+OSM_B200_API osm_b200_status osm_b200_plan_last_lld_launch(const osm_b200_plan *plan, const char **kernel, int32_t *grid,
+                                                           int64_t *n_chunks);
+
 #ifdef __cplusplus
 }
 #endif

@@ -270,6 +270,7 @@ EXPORTS = [
     "osm_b200_functionals_sizeof_spec",
     "osm_b200_plan_last_launch_count", "osm_b200_plan_take_device_flags", "osm_b200_plan_last_kernel_ms",
     "osm_b200_plan_last_kernel_times", "osm_b200_plan_set_profiling", "osm_b200_plan_profile_count", "osm_b200_plan_profile_entry",
+    "osm_b200_plan_last_lld_launch",
     # include/osm_b200_host.h
     "osm_b200_session_open", "osm_b200_session_close", "osm_b200_session_num_elements",
     "osm_b200_session_element_name", "osm_b200_session_extract_files", "osm_b200_session_extract_files_arff", "osm_b200_session_sink_options",
@@ -328,6 +329,7 @@ def lib():
     L.osm_b200_plan_set_profiling.restype = None
     L.osm_b200_plan_profile_count.argtypes = [vp]
     L.osm_b200_plan_profile_entry.argtypes = [vp, i32, C.POINTER(C.c_char_p), C.POINTER(C.c_float)]
+    L.osm_b200_plan_last_lld_launch.argtypes = [vp, C.POINTER(C.c_char_p), C.POINTER(i32), i64p]
     # host front end (include/osm_b200_host.h)
     cpp = C.POINTER(C.c_char_p)
     L.osm_b200_session_open.argtypes = [C.c_char_p, i32, cpp, cpp, C.c_char_p, i32, C.POINTER(vp)]

@@ -602,9 +602,11 @@ static void detect_fused_delta(osm_b200_plan *pl, bool simple)
                      g1.stages[0].flags == 0 && g2.stages[0].flags == 0 && g2.stages[1].flags == 0;   // plain regression only
   // OSM_B200_NO_FUSE=1 forces the two-kernel path (used by the tests to cross-check both)
   const char *nf = getenv("OSM_B200_NO_FUSE");
-  // the kernel keeps the statics of two tiles (2F frames): a row needs 2*halo+1 of them
+  // the kernel keeps the statics of two tiles (2F frames).  After a tile it emits the rows from hl before the tile's start to
+  // hl before its end; their delta-deltas read statics back to 2*hl before the tile's start, which the ring still holds
+  // only when 2*hl <= F (wider halos at 8- or 4-frame tiles run through post_kernel)
   const int hl = g1.stages[0].win + g2.stages[1].win, tF = pl->st[0].tileF;
-  if (shape && hl <= 8 && 2 * hl + 1 <= 2 * tF && !(nf && nf[0] == '1')) {
+  if (shape && hl <= 8 && 2 * hl <= tF && !(nf && nf[0] == '1')) {
     pl->fused = true;
     kp.fused = 1; kp.fW1 = g1.stages[0].win; kp.fW2 = g2.stages[1].win; kp.halo = kp.fW1 + kp.fW2;
     auto normOf = [](int W) { float n = 0.f; for (int i = 1; i <= W; i++) n += (float)i * (float)i; return n * 2.0f; };
@@ -1295,6 +1297,7 @@ osm_b200_status osm_b200_plan_run_device(osm_b200_plan *pl, const void *d_pcm, c
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   CU(cudaSetDevice(pl->device));
   pl->lastLaunches = 0;
+  pl->lastInfo = LldLaunchInfo{};
   pl->timed = false;
   pl->profN = 0;
   osm_b200_status s = prepare_batch(pl, utt_offsets, n_utt, frame_offsets, st);
@@ -1328,6 +1331,7 @@ static osm_b200_status run_host_impl(osm_b200_plan *pl, const void *pcm, const i
   }
   cudaStream_t st = pl->hostStream;
   pl->lastLaunches = 0;
+  pl->lastInfo = LldLaunchInfo{};
   pl->timed = false;
   osm_b200_status s = prepare_batch(pl, utt_offsets, n_utt, frame_offsets, st);
   if (s != OSM_B200_OK) return s;
@@ -1442,6 +1446,15 @@ osm_b200_status osm_b200_plan_copy_seq_lag(osm_b200_plan *pl, int32_t *out, int3
 }
 
 int32_t osm_b200_plan_last_launch_count(const osm_b200_plan *pl) { return pl ? pl->lastLaunches : 0; }
+
+osm_b200_status osm_b200_plan_last_lld_launch(const osm_b200_plan *pl, const char **kernel, int32_t *grid, int64_t *n_chunks)
+{
+  if (!pl) return fail(OSM_B200_ERR_INVALID, "null plan");
+  if (kernel) *kernel = pl->lastInfo.kernel;
+  if (grid) *grid = pl->lastInfo.grid;
+  if (n_chunks) *n_chunks = pl->lastInfo.nChunks;
+  return OSM_B200_OK;
+}
 
 int32_t osm_b200_plan_sample_frame_bytes(const osm_b200_plan *pl) { return pl ? pl->d.fe0().nChan * sample_bytes(pl->d.fe0().format) : 0; }
 

@@ -23,6 +23,7 @@
 // (which has no FMA contraction).  Only the FFT itself uses FMA freely.
 #include <cstdio>
 #include <cstdlib>
+#include <string>
 
 #include "fft_radix.cuh"
 #include "kernels.cuh"
@@ -86,7 +87,12 @@ __global__ void __launch_bounds__(NT, MINB) lld_kernel(const LldParams p)
     if (opKind == 1) for (int i = tid; i < p.nBands; i += NT) sEql[i] = p.plpEql[i];
     for (int i = tid; i < p.nStat; i += NT) sLift[i] = p.dctLift[i];
   }
-  for (int i = tid; i < L.sampFloats; i += NT) samp[i] = 0.f;   // lanes beyond a short tile read finite data
+  // Lanes beyond a short tile compute frames that are never stored, from the sample tile and from raw[] (the frames' first
+  // samples, written by the staging only for frames that start inside the tile).  Both start finite: the mel phase's
+  // zero-weight padding entries read up to three bins past the spectrum, which in P's storage (aliasing Z) hold FFT
+  // values of other lanes, and 0 * NaN would turn a valid frame's band into NaN.
+  for (int i = tid; i < L.sampFloats; i += NT) samp[i] = 0.f;
+  for (int i = tid; i < F; i += NT) raw[i] = 0.f;
   __syncthreads();
 
   const int hop = p.frameStep, nChan = p.nChan;
@@ -158,7 +164,8 @@ __global__ void __launch_bounds__(NT, MINB) lld_kernel(const LldParams p)
 #pragma unroll
           for (int jj = 0; jj < 8; jj++) y[jj] = x[jj];
         }
-        const int q = (int)__umulhi((unsigned)i, p.hopMagic);      // i / hop
+        // i / hop; the magic number of hop 1 (2^32) does not fit 32 bits
+        const int q = (hop == 1) ? i : (int)__umulhi((unsigned)i, p.hopMagic);
         const int r = i - q * hop;
         float *dst = samp + i + q * p.sPad;
         if (fastStore && nvalid == 8 && r + 8 <= hop) {
@@ -864,6 +871,18 @@ size_t lld_smem_bytes(const LldParams &p, int nfft)
   return (size_t)make_layout(p, nfft / 2, lld_tile_frames(nfft, p.narrow != 0)).total;
 }
 
+#define OSM_STR2(x) #x
+#define OSM_STR(x) OSM_STR2(x)
+// "lld_kernel<M,F,NT,MINB,VEC2|SCALAR,GEN|MFCC>" (lld_kernel_f32 in the float-input build), built once per instance
+template <int M, int F, int NT, int MINB, bool VEC2, bool GEN>
+static const char *lld_kernel_name()
+{
+  static const std::string name = std::string(OSM_STR(lld_kernel)) + "<" + std::to_string(M) + "," + std::to_string(F) + "," +
+                                  std::to_string(NT) + "," + std::to_string(MINB) + (VEC2 ? ",VEC2" : ",SCALAR") +
+                                  (GEN ? ",GEN>" : ",MFCC>");
+  return name.c_str();
+}
+
 template <int M, int F, int NT, int MINB, bool VEC2, bool GEN>
 static cudaError_t launch_g(const LldParams &p, int numSMs, cudaStream_t st, LldLaunchInfo *info)
 {
@@ -878,7 +897,10 @@ static cudaError_t launch_g(const LldParams &p, int numSMs, cudaStream_t st, Lld
   int grid = numSMs * occ;
   if (grid > p.nChunks) grid = p.nChunks;
   if (grid < 1) grid = 1;
-  if (info) { info->grid = grid; info->block = NT; info->smem = smem; }
+  if (info) {
+    info->grid = grid; info->block = NT; info->smem = smem; info->nChunks = p.nChunks;
+    info->kernel = lld_kernel_name<M, F, NT, MINB, VEC2, GEN>();
+  }
   kern<<<grid, NT, smem, st>>>(p);
   return cudaGetLastError();
 }

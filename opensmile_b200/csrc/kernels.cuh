@@ -79,6 +79,7 @@ struct LldParams {
   int pcmF32;
   // fused temporal stages (static | delta(W1) | delta(W1,W2)); halo = W1 + W2, 0 when not fused
   unsigned hopMagic;             // ceil(2^32 / frameStep): i / frameStep == __umulhi(i, hopMagic) for i * frameStep < 2^32
+                                 // (0 for frameStep 1: 2^32 does not fit)
   int narrow;                    // 1: half-width tiles (F/2 frames), used when the full tile does not fit shared memory
   int fused, halo, fW1, fW2;
   float fNorm1, fNorm2;
@@ -158,7 +159,8 @@ struct PostParams {
   const float *means;            // [nUtt][nStat] per-utterance column means (groups with a kind-2 stage), or null
 };
 
-struct LldLaunchInfo { int grid, block; size_t smem; };
+// kernel: static name of the instance that ran, e.g. "lld512_kernel<16>" or "lld_kernel<1024,8,256,1,VEC2,GEN>"
+struct LldLaunchInfo { int grid, block; size_t smem; const char *kernel; long long nChunks; };
 
 // returns cudaSuccess or the launch error; fills `info`
 cudaError_t launch_lld(const LldParams &p, int nfft, int numSMs, cudaStream_t st, LldLaunchInfo *info);

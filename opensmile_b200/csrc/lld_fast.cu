@@ -147,7 +147,9 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
     sDct[i] = (c < p.nStat) ? p.dctCos[c * p.dctStride + m] : 0.f;
   }
   for (int i = tid; i < p.nStat; i += NT) sLift[i] = p.dctLift[i];
+  // lanes beyond a short tile read finite data (see lld_kernel): the sample tile and the first samples of its frames
   for (int i = tid; i < L.sampFloats; i += NT) samp[i] = 0.f;
+  for (int i = tid; i < F; i += NT) raw[i] = 0.f;
   __syncthreads();
 
   const int hop = p.frameStep;
@@ -502,7 +504,10 @@ cudaError_t launch_fast_t(const LldParams &p, int numSMs, cudaStream_t st, LldLa
   int grid = numSMs * occ;
   if (grid > p.nChunks) grid = p.nChunks;
   if (grid < 1) grid = 1;
-  if (info) { info->grid = grid; info->block = kNT; info->smem = smem; }
+  if (info) {
+    info->grid = grid; info->block = kNT; info->smem = smem; info->nChunks = p.nChunks;
+    info->kernel = NZR == 13 ? "lld512_kernel<13>" : "lld512_kernel<16>";
+  }
   kern<<<grid, kNT, smem, st>>>(p);
   return cudaGetLastError();
 }

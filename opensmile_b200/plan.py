@@ -6,10 +6,13 @@ e.g. config/mfcc/MFCC12_0_D_A.conf).  torch is used only as the device-memory / 
 plumbing for the device-resident entry point.
 """
 import ctypes as C
+from collections import namedtuple
 
 import numpy as np
 
 from . import capi
+
+LldLaunch = namedtuple("LldLaunch", "kernel grid n_chunks")
 
 
 def _comp(ctype, name, reader, writer, **fields):
@@ -230,6 +233,12 @@ class Plan:
             raise RuntimeError(capi.last_error())
         return a.value, b.value
 
+    def last_lld_launch(self):
+        """(kernel instance name or None, grid, chunks) of the last per-frame kernel launch of the last run"""
+        nm, grid, n_chunks = C.c_char_p(), C.c_int32(0), C.c_int64(0)
+        if self._L.osm_b200_plan_last_lld_launch(self._h, C.byref(nm), C.byref(grid), C.byref(n_chunks)) != capi.OK:
+            raise RuntimeError(capi.last_error())
+        return LldLaunch(nm.value.decode() if nm.value else None, grid.value, n_chunks.value)
 
     def set_profiling(self, on):
         """per-kernel CUDA-event timing of run_device (serialises the step on one stream)"""
