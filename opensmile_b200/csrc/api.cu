@@ -12,6 +12,7 @@
 #include <string>
 #include <vector>
 
+#include "chunk_schedule.hpp"
 #include "cuda_owned.hpp"
 #include "kernels.cuh"
 #include "plan.hpp"
@@ -20,7 +21,7 @@ using namespace osm;
 
 // the _f32 builds of the PCM-reading launchers (kernels.cuh: OSM_F32_VARIANT), for plans whose input is not 16-bit integer
 namespace osm {
-cudaError_t launch_lld_f32(const LldParams &p, int nfft, int numSMs, cudaStream_t st, LldLaunchInfo *info);
+cudaError_t launch_lld_f32(const LldParams &p, int nfft, int numSMs, cudaStream_t st, LldLaunchInfo *info, bool launch = true);
 cudaError_t launch_energy_f32(const TimeOpParams &p, cudaStream_t st);
 cudaError_t launch_mzcr_f32(const TimeOpParams &p, cudaStream_t st);
 cudaError_t launch_intensity_f32(const TimeOpParams &p, cudaStream_t st);
@@ -126,7 +127,9 @@ struct StreamRt {
   bool needTiles = false;        // standalone ops read this stream tile by tile
   const float *dWindow = nullptr;   // [frameSize] window floats (time-domain ops)
   std::vector<int32_t> uttChunk0, uttTile0;
-  PinBuf<ChunkRef> hChunks; DevBuf<ChunkRef> dChunks; size_t nChunks = 0;
+  PinBuf<ChunkRef> hChunks; DevBuf<ChunkRef> dChunks; size_t nChunks = 0;   // + one entry whose w0 ends the schedule
+  int lldCtas = 1;               // CTAs pass 0's lld instance keeps resident
+  int ctaTiles = 1;              // tiles per CTA run of the whole batch (LldParams::ctaTiles)
   PinBuf<OpTile> hTiles; DevBuf<OpTile> dTiles; size_t nTiles = 0;
   DevBuf<float> dMag;
 };
@@ -1017,38 +1020,34 @@ static osm_b200_status prepare_batch(osm_b200_plan *pl, const int64_t *uttOff, i
       std::vector<ChunkRef> chunks;
       std::vector<OpTile> tiles;
       rt.uttChunk0.assign(nm, 0); rt.uttTile0.assign(nm, 0);
-      int64_t tileCount = 0;
-      for (int u = 0; u < nUtt; u++) {
-        const int64_t L = uttOff[u + 1] - uttOff[u];
-        const int64_t T = desc_num_static_frames(d, (int)si, L);
-        rt.uttChunk0[u] = (int32_t)chunks.size();
-        rt.uttTile0[u] = (int32_t)tileCount;
-        // chunks: output rows [a,b) whose static range [a-H, b+H) /\ [0,T) is a whole number of
-        // tiles (except at the utterance end), at most KT tiles each
-        for (int64_t a = 0; a < T;) {
-          const int64_t s0 = std::max<int64_t>(a - H, 0);
-          const int64_t maxEnd = s0 + (int64_t)F * KT;
-          const int64_t b2 = (maxEnd >= T) ? T : maxEnd - H;
-          chunks.push_back(ChunkRef{u, (int32_t)a, (int32_t)b2, (int32_t)(tileCount + s0 / F)});
-          a = b2;
-        }
-        if (rt.needTiles)
-          for (int64_t f0 = 0; f0 < T; f0 += F)
-            tiles.push_back(OpTile{u, (int32_t)f0, (int32_t)std::min<int64_t>(F, T - f0), f0 > 0 ? 1 : 0});
-        tileCount += (T + F - 1) / F;
+      std::vector<int64_t> T(nUtt);
+      for (int u = 0; u < nUtt; u++) T[u] = desc_num_static_frames(d, (int)si, uttOff[u + 1] - uttOff[u]);
+      if (rt.runLld) {
+        // one run of chunks per resident CTA of the instance the launch will select (same parameters as launch_range)
+        cut_chunks(T.data(), nUtt, F, H, KT, 0, chunks, rt.uttChunk0.data(), rt.uttTile0.data());
+        if (rt.kp.opKind < 0 || d.streams[si].dumpMag)
+          CU(rt.dMag.reserve((size_t)rt.uttTile0[nUtt] * d.streams[si].fe.nBins * F + 64));
+        LldParams kq = rt.kp;
+        kq.magOut = d.streams[si].dumpMag ? rt.dMag.p : nullptr;
+        LldLaunchInfo li{};
+        CU((d.fe0().format != OSM_B200_PCM_S16 ? launch_lld_f32 : launch_lld)(kq, d.streams[si].fe.nfft, pl->numSMs, st, &li, false));
+        rt.lldCtas = std::max(li.grid, 1);
+        rt.ctaTiles = (int)balanced_chunks(T.data(), nUtt, F, H, KT, rt.lldCtas, chunks, rt.uttChunk0.data(), rt.uttTile0.data());
+      } else {
+        cut_chunks(T.data(), nUtt, F, H, KT, 0, chunks, rt.uttChunk0.data(), rt.uttTile0.data());
       }
-      rt.uttChunk0[nUtt] = (int32_t)chunks.size();
-      rt.uttTile0[nUtt] = (int32_t)tileCount;
-      rt.nChunks = rt.runLld ? chunks.size() : 0;
+      if (rt.needTiles)
+        for (int u = 0; u < nUtt; u++)
+          for (int64_t f0 = 0; f0 < T[u]; f0 += F)
+            tiles.push_back(OpTile{u, (int32_t)f0, (int32_t)std::min<int64_t>(F, T[u] - f0), f0 > 0 ? 1 : 0});
+      rt.nChunks = rt.runLld ? chunks.size() - 1 : 0;
       rt.nTiles = tiles.size();
       pl->totalWork += rt.nChunks + rt.nTiles;
       if (rt.runLld) {
-        CU(rt.hChunks.reserve(chunks.size() + 1));
-        if (!chunks.empty()) memcpy(rt.hChunks.p, chunks.data(), chunks.size() * sizeof(ChunkRef));
-        CU(rt.dChunks.reserve(chunks.size() + 1));
-        if (!chunks.empty()) CU(cudaMemcpyAsync(rt.dChunks.p, rt.hChunks.p, chunks.size() * sizeof(ChunkRef), cudaMemcpyHostToDevice, st));
-        if (rt.kp.opKind < 0 || d.streams[si].dumpMag)
-          CU(rt.dMag.reserve((size_t)tileCount * d.streams[si].fe.nBins * F + 64));
+        CU(rt.hChunks.reserve(chunks.size()));
+        memcpy(rt.hChunks.p, chunks.data(), chunks.size() * sizeof(ChunkRef));
+        CU(rt.dChunks.reserve(chunks.size()));
+        CU(cudaMemcpyAsync(rt.dChunks.p, rt.hChunks.p, chunks.size() * sizeof(ChunkRef), cudaMemcpyHostToDevice, st));
       }
       if (rt.needTiles) {
         CU(rt.hTiles.reserve(tiles.size() + 1));
@@ -1131,6 +1130,13 @@ static osm_b200_status launch_range(osm_b200_plan *pl, const void *d_pcm, float 
       kp.uttOff = dU;
       kp.chunks = rt.dChunks.p + c0;
       kp.nChunks = c1 - c0;
+      {
+        // the whole batch runs the schedule prepare_batch cut; a part of it (run_host's pieces) is dealt over the
+        // resident CTAs in runs of whole chunks
+        const int64_t W = rt.hChunks.p[c1].w0 - rt.hChunks.p[c0].w0;
+        kp.ctaTiles = (c0 == 0 && c1 == (int)rt.nChunks) ? rt.ctaTiles : (int)((W + rt.lldCtas - 1) / rt.lldCtas);
+        kp.nRuns = (int)((W + kp.ctaTiles - 1) / kp.ctaTiles);
+      }
       kp.magOut = (j == 0 && d.streams[si].dumpMag) ? rt.dMag.p : nullptr;
       if (pl->staticDirect) {
         kp.out = d_out; kp.outStride = d.nOut; kp.outCol = pl->identityOutCol; kp.rowOff = dR;
@@ -1142,7 +1148,7 @@ static osm_b200_status launch_range(osm_b200_plan *pl, const void *d_pcm, float 
         CU(pr.dBand.reserve((size_t)pl->totalStat * kp.nBands + 64));
         kp.out = pr.dBand.p; kp.outStride = kp.nBands; kp.outCol = 0; kp.rowOff = dS;
       }
-      CU((f32in ? launch_lld_f32 : launch_lld)(kp, d.streams[si].fe.nfft, pl->numSMs, st, &pl->lastInfo));
+      CU((f32in ? launch_lld_f32 : launch_lld)(kp, d.streams[si].fe.nfft, pl->numSMs, st, &pl->lastInfo, true));
       pl->lastLaunches++;
       PROF("lld_kernel");
       if (pr.rasta) {

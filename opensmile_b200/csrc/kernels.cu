@@ -75,8 +75,10 @@ __global__ void __launch_bounds__(NT, MINB) lld_kernel(const LldParams p)
   const int f = lane & (F - 1);
   const int vw = warp * G + lane / F;
 
-  // ---- one-time setup: barrier, constant tables -> smem, zero the sample tile ----
+  // ---- one-time setup: barrier, this CTA's chunks [sRun[0], sRun[1]), constant tables -> smem, zero the sample tile ----
+  __shared__ int sRun[2];
   if (tid == 0) mbar_init(mbar, 1);
+  if (tid < 2) sRun[tid] = chunk_run_begin(p, blockIdx.x + tid);
   for (int i = tid; i < M; i += NT) sWinLut[i] = p.winLut[i];
   for (int i = tid; i < p.twCount; i += NT) sTw[i] = p.twiddles[i];
   for (int i = tid; i < NPAIR; i += NT) sSplit[i] = p.splitTw[i];
@@ -99,8 +101,9 @@ __global__ void __launch_bounds__(NT, MINB) lld_kernel(const LldParams p)
   const int S = hop + p.sPad;
   uint32_t phase = 0;
 
-  int chunk = blockIdx.x;
-  if (chunk >= p.nChunks) return;
+  int chunk = sRun[0];
+  const int chunkEnd = sRun[1];
+  if (chunk >= chunkEnd) return;
   ChunkCtx cx = load_chunk<F>(p, chunk);
   int j = 0;
   int emitted = cx.a;                 // next output row of the current chunk to be written
@@ -110,7 +113,7 @@ __global__ void __launch_bounds__(NT, MINB) lld_kernel(const LldParams p)
     bulk_g2s(rawPcm, g0.src, g0.bytes, mbar);
   }
 
-  while (chunk < p.nChunks) {
+  while (chunk < chunkEnd) {
     const TileGeom tg = tile_geom<F>(p, cx, j);
     const int nf = tg.nf, count = tg.count;
 
@@ -194,8 +197,8 @@ __global__ void __launch_bounds__(NT, MINB) lld_kernel(const LldParams p)
         const TileGeom gn = tile_geom<F>(p, cx, j + 1);
         mbar_expect_tx(mbar, gn.bytes);
         bulk_g2s(rawPcm, gn.src, gn.bytes, mbar);
-      } else if (chunk + (int)gridDim.x < p.nChunks) {
-        const ChunkCtx cn = load_chunk<F>(p, chunk + gridDim.x);
+      } else if (chunk + 1 < chunkEnd) {
+        const ChunkCtx cn = load_chunk<F>(p, chunk + 1);
         const TileGeom gn = tile_geom<F>(p, cn, 0);
         mbar_expect_tx(mbar, gn.bytes);
         bulk_g2s(rawPcm, gn.src, gn.bytes, mbar);
@@ -439,9 +442,9 @@ __global__ void __launch_bounds__(NT, MINB) lld_kernel(const LldParams p)
     // ---- advance to the next tile / chunk ----
     j++;
     if (j == cx.nT) {
-      chunk += gridDim.x;
+      chunk++;
       j = 0;
-      if (chunk < p.nChunks) { cx = load_chunk<F>(p, chunk); emitted = cx.a; }
+      if (chunk < chunkEnd) { cx = load_chunk<F>(p, chunk); emitted = cx.a; }
     }
   }
 }
@@ -884,7 +887,7 @@ static const char *lld_kernel_name()
 }
 
 template <int M, int F, int NT, int MINB, bool VEC2, bool GEN>
-static cudaError_t launch_g(const LldParams &p, int numSMs, cudaStream_t st, LldLaunchInfo *info)
+static cudaError_t launch_g(const LldParams &p, int numSMs, cudaStream_t st, LldLaunchInfo *info, bool launch)
 {
   const size_t smem = (size_t)make_layout(p, M, F).total;
   auto kern = lld_kernel<M, F, NT, MINB, VEC2, GEN>;
@@ -894,41 +897,40 @@ static cudaError_t launch_g(const LldParams &p, int numSMs, cudaStream_t st, Lld
   e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, NT, smem);
   if (e != cudaSuccess) return e;
   if (occ < 1) return cudaErrorLaunchOutOfResources;
-  int grid = numSMs * occ;
-  if (grid > p.nChunks) grid = p.nChunks;
-  if (grid < 1) grid = 1;
+  const int grid = launch ? p.nRuns : numSMs * occ;
   if (info) {
     info->grid = grid; info->block = NT; info->smem = smem; info->nChunks = p.nChunks;
     info->kernel = lld_kernel_name<M, F, NT, MINB, VEC2, GEN>();
   }
+  if (!launch) return cudaSuccess;
   kern<<<grid, NT, smem, st>>>(p);
   return cudaGetLastError();
 }
 
 template <int M, int F, int NT, int MINB, bool VEC2>
-static cudaError_t launch_t(const LldParams &p, int numSMs, cudaStream_t st, LldLaunchInfo *info)
+static cudaError_t launch_t(const LldParams &p, int numSMs, cudaStream_t st, LldLaunchInfo *info, bool launch)
 {
-  if (p.opKind == 0 && p.magOut == nullptr) return launch_g<M, F, NT, MINB, VEC2, false>(p, numSMs, st, info);
-  return launch_g<M, F, NT, MINB, VEC2, true>(p, numSMs, st, info);
+  if (p.opKind == 0 && p.magOut == nullptr) return launch_g<M, F, NT, MINB, VEC2, false>(p, numSMs, st, info, launch);
+  return launch_g<M, F, NT, MINB, VEC2, true>(p, numSMs, st, info, launch);
 }
 
-cudaError_t launch_lld(const LldParams &p, int nfft, int numSMs, cudaStream_t st, LldLaunchInfo *info)
+cudaError_t launch_lld(const LldParams &p, int nfft, int numSMs, cudaStream_t st, LldLaunchInfo *info, bool launch)
 {
   {
     static const bool fastOn = [] { const char *e = getenv("OSM_B200_LLD_FAST"); return !(e && e[0] == '0'); }();
-    if (fastOn && lld_fast_applies(p, nfft)) return launch_lld_fast(p, numSMs, st, info);
+    if (fastOn && lld_fast_applies(p, nfft)) return launch_lld_fast(p, numSMs, st, info, launch);
   }
   // VEC2: 64-bit sample-pair loads need an even per-lane stride (frameStep + sPad)
   const bool vec2 = ((p.frameStep + p.sPad) % 2) == 0;
   // narrow tiles: half the frames per tile with half the threads (same number of virtual warps)
-  if (p.narrow && nfft == 1024) return vec2 ? launch_t<512, 16, 256, 1, true>(p, numSMs, st, info) : launch_t<512, 16, 256, 1, false>(p, numSMs, st, info);
-  if (p.narrow && nfft == 2048) return vec2 ? launch_t<1024, 8, 256, 1, true>(p, numSMs, st, info) : launch_t<1024, 8, 256, 1, false>(p, numSMs, st, info);
-  if (p.narrow && nfft == 4096) return vec2 ? launch_t<2048, 4, 128, 1, true>(p, numSMs, st, info) : launch_t<2048, 4, 128, 1, false>(p, numSMs, st, info);
+  if (p.narrow && nfft == 1024) return vec2 ? launch_t<512, 16, 256, 1, true>(p, numSMs, st, info, launch) : launch_t<512, 16, 256, 1, false>(p, numSMs, st, info, launch);
+  if (p.narrow && nfft == 2048) return vec2 ? launch_t<1024, 8, 256, 1, true>(p, numSMs, st, info, launch) : launch_t<1024, 8, 256, 1, false>(p, numSMs, st, info, launch);
+  if (p.narrow && nfft == 4096) return vec2 ? launch_t<2048, 4, 128, 1, true>(p, numSMs, st, info, launch) : launch_t<2048, 4, 128, 1, false>(p, numSMs, st, info, launch);
   switch (nfft) {
-    case 512:  return vec2 ? launch_t<256, 32, 256, 2, true>(p, numSMs, st, info) : launch_t<256, 32, 256, 2, false>(p, numSMs, st, info);
-    case 1024: return vec2 ? launch_t<512, 32, 512, 1, true>(p, numSMs, st, info) : launch_t<512, 32, 512, 1, false>(p, numSMs, st, info);
-    case 2048: return vec2 ? launch_t<1024, 16, 512, 1, true>(p, numSMs, st, info) : launch_t<1024, 16, 512, 1, false>(p, numSMs, st, info);
-    case 4096: return vec2 ? launch_t<2048, 8, 256, 1, true>(p, numSMs, st, info) : launch_t<2048, 8, 256, 1, false>(p, numSMs, st, info);
+    case 512:  return vec2 ? launch_t<256, 32, 256, 2, true>(p, numSMs, st, info, launch) : launch_t<256, 32, 256, 2, false>(p, numSMs, st, info, launch);
+    case 1024: return vec2 ? launch_t<512, 32, 512, 1, true>(p, numSMs, st, info, launch) : launch_t<512, 32, 512, 1, false>(p, numSMs, st, info, launch);
+    case 2048: return vec2 ? launch_t<1024, 16, 512, 1, true>(p, numSMs, st, info, launch) : launch_t<1024, 16, 512, 1, false>(p, numSMs, st, info, launch);
+    case 4096: return vec2 ? launch_t<2048, 8, 256, 1, true>(p, numSMs, st, info, launch) : launch_t<2048, 8, 256, 1, false>(p, numSMs, st, info, launch);
     default:   return cudaErrorInvalidValue;
   }
 }

@@ -62,7 +62,9 @@ namespace osm {
 constexpr int kMaxVW = 32;   // virtual warps (F-lane groups) per CTA
 
 struct TileRef { int32_t utt; int32_t f0; };   // (utterance, first row) of a post_kernel tile
-struct ChunkRef { int32_t utt; int32_t a; int32_t b; int32_t tile0; };   // output rows [a,b) of one utterance = one CTA work unit; tile0 = global index of its first tile
+// output rows [a,b) of one utterance = one CTA work unit; tile0 = global index of its first tile; w0 = tiles the chunks
+// before it in the list compute (the position of its first tile in the launch's schedule, see LldParams::ctaTiles)
+struct ChunkRef { int32_t utt; int32_t a; int32_t b; int32_t tile0; int32_t w0; };
 
 // Everything the fused per-frame kernel needs.  Pointers are device pointers; the table
 // pointers reference one packed constant blob uploaded at plan creation.
@@ -73,6 +75,9 @@ struct LldParams {
   const long long *rowOff;       // [nUtt+1] first output row of each utterance
   const ChunkRef *chunks;
   int nChunks;
+  // schedule: CTA g runs, in order, the chunks c with g * ctaTiles <= chunks[c].w0 - chunks[0].w0 < (g + 1) * ctaTiles,
+  // a contiguous run of about ctaTiles tiles (the host cuts chunks at these boundaries); nRuns = grid size
+  int ctaTiles, nRuns;
   int nChan;
   // 1: `pcm` holds pre-converted mono float samples (pcm_convert_kernel: every input format but 16-bit integer).  The sample
   // frame is 4 bytes wide, so nChan is 2 here -- all offset arithmetic stays in int16 units -- and only the conversion differs.
@@ -162,13 +167,14 @@ struct PostParams {
 // kernel: static name of the instance that ran, e.g. "lld512_kernel<16>" or "lld_kernel<1024,8,256,1,VEC2,GEN>"
 struct LldLaunchInfo { int grid, block; size_t smem; const char *kernel; long long nChunks; };
 
-// returns cudaSuccess or the launch error; fills `info`
-cudaError_t launch_lld(const LldParams &p, int nfft, int numSMs, cudaStream_t st, LldLaunchInfo *info);
+// returns cudaSuccess or the launch error; fills `info`.  launch = false only fills `info`, with grid = the CTAs the
+// selected instance keeps resident (numSMs x occupancy)
+cudaError_t launch_lld(const LldParams &p, int nfft, int numSMs, cudaStream_t st, LldLaunchInfo *info, bool launch = true);
 cudaError_t launch_post(const PostParams &p, cudaStream_t st);
 // lld_fast.cu: the specialised 512-point mono MFCC instance (same contract and results as lld_kernel); launch_lld selects it
 // unless OSM_B200_LLD_FAST=0
 bool lld_fast_applies(const LldParams &p, int nfft);
-cudaError_t launch_lld_fast(const LldParams &p, int numSMs, cudaStream_t st, LldLaunchInfo *info);
+cudaError_t launch_lld_fast(const LldParams &p, int numSMs, cudaStream_t st, LldLaunchInfo *info, bool launch);
 // output rows per post_kernel CTA: 64, or fewer when a wide static level would not fit shared memory
 int post_tile_rows(int nStat, int maxN, int halo);
 // smem bytes the fused kernel needs for a given geometry (host helper, used for diagnostics)

@@ -163,6 +163,19 @@ __device__ __forceinline__ ChunkCtx load_chunk(const LldParams &p, int chunk)
   return c;
 }
 
+// first chunk of CTA g's run (LldParams::ctaTiles): the first chunk whose schedule position is at least g * ctaTiles
+__device__ __forceinline__ int chunk_run_begin(const LldParams &p, int g)
+{
+  const long long w = (long long)p.chunks[0].w0 + (long long)g * p.ctaTiles;
+  int lo = 0, hi = p.nChunks;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (p.chunks[mid].w0 < w) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
 // geometry of one tile (all warp-uniform)
 struct TileGeom {
   int fs;            // first static frame of the tile

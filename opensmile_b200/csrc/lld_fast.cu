@@ -50,6 +50,27 @@
 #define OSM_UNROLL(n) OSM_PRAGMA_(unroll n)
 
 namespace osm {
+
+// Phase clocks (build with -DOSM_LLD_PHASE_CLOCKS, `make phase-clocks`; off in the default library): thread 0 of every CTA
+// reads clock64() at each phase boundary of every tile and adds the cycles since the previous boundary into a per-CTA slot;
+// the CTA's sums go to gLld512Phase at its exit.  Most boundaries follow a barrier, so a phase's count is the CTA's time
+// from one barrier to the next.  Emit and store end without one: they count thread 0's own share, and the wait for the
+// other threads lands in the next tile's stage.  scripts/lld512_phase_clocks.py prints the sums per frame.
+enum { kPhStage, kPhPass1, kPhPass2, kPhMel, kPhDct, kPhEmit, kPhStore, kPhKernel, kPhKernelMax, kPhTiles, kPhSlots };
+#ifdef OSM_LLD_PHASE_CLOCKS
+__device__ unsigned long long gLld512Phase[kPhSlots];
+#define OSM_PHASE(k)                                                    \
+  do {                                                                  \
+    if (tid == 0) {                                                     \
+      const long long c_ = clock64();                                   \
+      sPh[k] += (unsigned long long)(c_ - phT);                         \
+      phT = c_;                                                         \
+    }                                                                   \
+  } while (0)
+#else
+#define OSM_PHASE(k) do {} while (0)
+#endif
+
 namespace {
 
 constexpr int kM = 256, kF = 32, kNT = 256, kNW = 8;
@@ -116,6 +137,7 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
 
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ ChunkCtx sCx[2];
+  __shared__ int sRun[2];
   const SmemLayout L = make_layout(p, M, F);
   float2 *Z = reinterpret_cast<float2 *>(smem + L.zbuf);
   float *P = reinterpret_cast<float *>(smem + L.zbuf);
@@ -137,6 +159,7 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
   const int warp = tid >> 5, f = tid & 31;
 
   if (tid == 0) mbar_init(mbar, 1);
+  if (tid < 2) sRun[tid] = chunk_run_begin(p, blockIdx.x + tid);   // this CTA's chunks: [sRun[0], sRun[1])
   for (int i = tid; i < M; i += NT) sWinLut[i] = p.winLut[i];
   for (int i = tid; i < p.twCount; i += NT) sTw[i] = p.twiddles[i];
   for (int i = tid; i < M / 2 + 1; i += NT) sSplit[i] = p.splitTw[i];
@@ -155,11 +178,18 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
   const int hop = p.frameStep;
   const int S = hop + p.sPad;
   uint32_t phase = 0;
+#ifdef OSM_LLD_PHASE_CLOCKS
+  __shared__ unsigned long long sPh[kPhSlots];
+  if (tid < kPhSlots) sPh[tid] = 0;
+  const long long phT0 = clock64();
+  long long phT = phT0;
+#endif
 
   // The chunk context is CTA-uniform: it lives in shared memory (current / next chunk, alternating) instead of a dozen
   // registers per thread; thread 0 fills the next slot when it prefetches that chunk's first tile.
-  int chunk = blockIdx.x;
-  if (chunk >= p.nChunks) return;
+  int chunk = sRun[0];
+  const int chunkEnd = sRun[1];
+  if (chunk >= chunkEnd) return;
   int cpar = 0;
   if (tid == 0) {
     sCx[0] = load_chunk<F>(p, chunk);
@@ -178,7 +208,7 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
   const int wl = (warp == 0) ? 8 : warp, wh = (warp == 0) ? 0 : warp;
   const int melBs = p.melSplit[warp], melBe = p.melSplit[warp + 1];
 
-  while (chunk < p.nChunks) {
+  while (chunk < chunkEnd) {
     const ChunkCtx &cx = sCx[cpar];
 
     // ================= stage: PCM (landing zone) -> float -> pre-emphasis -> sample tile =================
@@ -231,14 +261,15 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
         const TileGeom gn = tile_geom<F>(p, cx, j + 1);
         mbar_expect_tx(mbar, gn.bytes);
         bulk_g2s(rawPcm, gn.src, gn.bytes, mbar);
-      } else if (chunk + (int)gridDim.x < p.nChunks) {
-        const ChunkCtx cn = load_chunk<F>(p, chunk + gridDim.x);
+      } else if (chunk + 1 < chunkEnd) {
+        const ChunkCtx cn = load_chunk<F>(p, chunk + 1);
         sCx[cpar ^ 1] = cn;                           // read by everyone after the barriers of this tile
         const TileGeom gn = tile_geom<F>(p, cn, 0);
         mbar_expect_tx(mbar, gn.bytes);
         bulk_g2s(rawPcm, gn.src, gn.bytes, mbar);
       }
     }
+    OSM_PHASE(kPhStage);
 
     // ================= FFT pass 1: window, radix 16, twiddles -> Z =================
     {
@@ -269,6 +300,7 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
       }
     }
     __syncthreads();
+    OSM_PHASE(kPhPass1);
 
     // ================= FFT pass 2 + real-FFT split + power, in registers =================
     {
@@ -326,6 +358,7 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
       }
     }
     __syncthreads();
+    OSM_PHASE(kPhPass2);
 
 #if OSM_FAST_FUSED_DCT
     // ================= mel filterbank (melspec.cpp:543-569) + log (mfcc.cpp:239-243) + DCT-II partial sums =================
@@ -375,6 +408,7 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
       for (int c = 0; c < kKMax; c++) part[c * F] = acc[c];
     }
     __syncthreads();
+    OSM_PHASE(kPhMel);
 
     // ================= DCT-II: sum of the warps' partial sums, lifter (mfcc.cpp:268-272) =================
     const int ringBase = (j & 1) * F;
@@ -386,6 +420,7 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
       ring[c * (2 * F) + ringBase + f] = __fmul_rn(a, sLift[c]);
     }
     __syncthreads();
+    OSM_PHASE(kPhDct);
 
 #else
     // ================= mel filterbank (melspec.cpp:543-569) + log (mfcc.cpp:239-243) =================
@@ -417,6 +452,7 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
       }
     }
     __syncthreads();
+    OSM_PHASE(kPhMel);
 
     // ================= DCT-II + lifter (mfcc.cpp:251-272), the reference's m = 0 .. nBands-1 accumulation order =================
     // table transposed and zero padded, sDct[band][kKMax]: warp w evaluates coefficients 2w and 2w+1 together (one 8-byte
@@ -439,6 +475,7 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
       }
     }
     __syncthreads();
+    OSM_PHASE(kPhDct);
 
 #endif
     // ================= store (same statements as lld_kernel) =================
@@ -472,6 +509,7 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
       } else {
         emit_edge<F, NW>(ring, Dbuf, outS, K, W1, W2, T, T1, c01, c02, cx.s0, r0, r1, d0, d1, dRows, norm1, p.fRcp1, norm2, p.fRcp2, warp, f);
       }
+      OSM_PHASE(kPhEmit);
       {
         float *o = p.out + (cx.row0 + r0) * (long long)K3;
         const int n = nr * K3;
@@ -479,19 +517,31 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
       }
       emitted = r1;
     }
+    OSM_PHASE(kPhStore);
+#ifdef OSM_LLD_PHASE_CLOCKS
+    if (tid == 0) sPh[kPhTiles]++;
+#endif
 
     j++;
     if (j == cx.nT) {
-      chunk += gridDim.x;
+      chunk++;
       j = 0;
       cpar ^= 1;
-      if (chunk < p.nChunks) emitted = sCx[cpar].a;
+      if (chunk < chunkEnd) emitted = sCx[cpar].a;
     }
   }
+#ifdef OSM_LLD_PHASE_CLOCKS
+  if (tid == 0) {
+    sPh[kPhKernel] = (unsigned long long)(clock64() - phT0);
+    for (int k = 0; k < kPhSlots; k++)
+      if (k != kPhKernelMax) atomicAdd(&gLld512Phase[k], sPh[k]);
+    atomicMax(&gLld512Phase[kPhKernelMax], sPh[kPhKernel]);
+  }
+#endif
 }
 
 template <int NZR>
-cudaError_t launch_fast_t(const LldParams &p, int numSMs, cudaStream_t st, LldLaunchInfo *info)
+cudaError_t launch_fast_t(const LldParams &p, int numSMs, cudaStream_t st, LldLaunchInfo *info, bool launch)
 {
   const size_t smem = (size_t)make_layout(p, kM, kF).total;
   auto kern = lld512_kernel<NZR>;
@@ -501,13 +551,12 @@ cudaError_t launch_fast_t(const LldParams &p, int numSMs, cudaStream_t st, LldLa
   e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kNT, smem);
   if (e != cudaSuccess) return e;
   if (occ < 1) return cudaErrorLaunchOutOfResources;
-  int grid = numSMs * occ;
-  if (grid > p.nChunks) grid = p.nChunks;
-  if (grid < 1) grid = 1;
+  const int grid = launch ? p.nRuns : numSMs * occ;
   if (info) {
     info->grid = grid; info->block = kNT; info->smem = smem; info->nChunks = p.nChunks;
     info->kernel = NZR == 13 ? "lld512_kernel<13>" : "lld512_kernel<16>";
   }
+  if (!launch) return cudaSuccess;
   kern<<<grid, kNT, smem, st>>>(p);
   return cudaGetLastError();
 }
@@ -521,10 +570,23 @@ bool lld_fast_applies(const LldParams &p, int nfft)
          ((p.frameStep + p.sPad) % 2) == 0;
 }
 
-cudaError_t launch_lld_fast(const LldParams &p, int numSMs, cudaStream_t st, LldLaunchInfo *info)
+cudaError_t launch_lld_fast(const LldParams &p, int numSMs, cudaStream_t st, LldLaunchInfo *info, bool launch)
 {
-  if (p.frameSize <= 416) return launch_fast_t<13>(p, numSMs, st, info);
-  return launch_fast_t<16>(p, numSMs, st, info);
+  if (p.frameSize <= 416) return launch_fast_t<13>(p, numSMs, st, info, launch);
+  return launch_fast_t<16>(p, numSMs, st, info, launch);
 }
+
+#ifdef OSM_LLD_PHASE_CLOCKS
+// copies the phase sums of every launch since the previous call into out[kPhSlots] and clears them
+extern "C" __attribute__((visibility("default"))) int osm_b200_lld512_phase_clocks(unsigned long long *out)
+{
+  cudaError_t e = cudaMemcpyFromSymbol(out, gLld512Phase, sizeof(gLld512Phase));
+  if (e == cudaSuccess) {
+    static const unsigned long long zero[kPhSlots] = {};
+    e = cudaMemcpyToSymbol(gLld512Phase, zero, sizeof(zero));
+  }
+  return (int)e;
+}
+#endif
 
 }  // namespace osm
