@@ -19,18 +19,6 @@
 
 using namespace osm;
 
-// the _f32 builds of the PCM-reading launchers (kernels.cuh: OSM_F32_VARIANT), for plans whose input is not 16-bit integer
-namespace osm {
-cudaError_t launch_lld_f32(const LldParams &p, int nfft, int numSMs, cudaStream_t st, LldLaunchInfo *info, bool launch = true);
-cudaError_t launch_energy_f32(const TimeOpParams &p, cudaStream_t st);
-cudaError_t launch_mzcr_f32(const TimeOpParams &p, cudaStream_t st);
-cudaError_t launch_intensity_f32(const TimeOpParams &p, cudaStream_t st);
-cudaError_t launch_formant_f32(const FormantParams &p, cudaStream_t st);
-cudaError_t launch_lpc_f32(const LpcParams &p, cudaStream_t st);
-size_t lpc_smem_bytes_f32(const LpcParams &p);
-cudaError_t launch_jitter_f32(const JitterParams &p, int u0, int u1, cudaStream_t st);
-}
-
 namespace {
 thread_local std::string g_err;
 }
@@ -1030,7 +1018,7 @@ static osm_b200_status prepare_batch(osm_b200_plan *pl, const int64_t *uttOff, i
         LldParams kq = rt.kp;
         kq.magOut = d.streams[si].dumpMag ? rt.dMag.p : nullptr;
         LldLaunchInfo li{};
-        CU((d.fe0().format != OSM_B200_PCM_S16 ? launch_lld_f32 : launch_lld)(kq, d.streams[si].fe.nfft, pl->numSMs, st, &li, false));
+        CU(launch_lld(kq, d.streams[si].fe.nfft, pl->numSMs, st, &li, false));
         rt.lldCtas = std::max(li.grid, 1);
         rt.ctaTiles = (int)balanced_chunks(T.data(), nUtt, F, H, KT, rt.lldCtas, chunks, rt.uttChunk0.data(), rt.uttTile0.data());
       } else {
@@ -1148,7 +1136,7 @@ static osm_b200_status launch_range(osm_b200_plan *pl, const void *d_pcm, float 
         CU(pr.dBand.reserve((size_t)pl->totalStat * kp.nBands + 64));
         kp.out = pr.dBand.p; kp.outStride = kp.nBands; kp.outCol = 0; kp.rowOff = dS;
       }
-      CU((f32in ? launch_lld_f32 : launch_lld)(kp, d.streams[si].fe.nfft, pl->numSMs, st, &pl->lastInfo, true));
+      CU(launch_lld(kp, d.streams[si].fe.nfft, pl->numSMs, st, &pl->lastInfo, true));
       pl->lastLaunches++;
       PROF("lld_kernel");
       if (pr.rasta) {
@@ -1216,7 +1204,7 @@ static osm_b200_status launch_range(osm_b200_plan *pl, const void *d_pcm, float 
       JitterParams jp = o.jit;
       jp.pcm = reinterpret_cast<const int16_t *>(d_pcm);
       jp.uttOff = dU; jp.statOff = dS; jp.stat = pl->dStat.p; jp.errFlag = pl->dErr.p;
-      CU((f32in ? launch_jitter_f32 : launch_jitter)(jp, u0, u1, ks));
+      CU(launch_jitter(jp, u0, u1, ks));
       PROF("jitter_kernel");
     } else if (o.kind == SOP_PITCHACF) {
       AcfPitchParams ap = o.ap;
@@ -1235,11 +1223,10 @@ static osm_b200_status launch_range(osm_b200_plan *pl, const void *d_pcm, float 
       tp.uttOff = dU; tp.statOff = dS;
       tp.tiles = rt.dTiles.p + t0; tp.nTiles = t1 - t0;
       tp.stat = pl->dStat.p;
-      if (o.kind == SOP_FORMANT) { FormantParams fp = o.fmt; fp.tp = tp; CU((f32in ? launch_formant_f32 : launch_formant)(fp, st)); PROF("formant_kernel"); }
-      else if (o.kind == SOP_LPC) { LpcParams lp = o.lpc; lp.tp = tp; CU((f32in ? launch_lpc_f32 : launch_lpc)(lp, st)); PROF("lpc_kernel"); }
+      if (o.kind == SOP_FORMANT) { FormantParams fp = o.fmt; fp.tp = tp; CU(launch_formant(fp, st)); PROF("formant_kernel"); }
+      else if (o.kind == SOP_LPC) { LpcParams lp = o.lpc; lp.tp = tp; CU(launch_lpc(lp, st)); PROF("lpc_kernel"); }
       else {
-        CU(o.kind == SOP_ENERGY ? (f32in ? launch_energy_f32 : launch_energy)(tp, st)
-                                : (o.kind == SOP_INTENSITY ? (f32in ? launch_intensity_f32 : launch_intensity)(tp, st) : (f32in ? launch_mzcr_f32 : launch_mzcr)(tp, st)));
+        CU(o.kind == SOP_ENERGY ? launch_energy(tp, st) : (o.kind == SOP_INTENSITY ? launch_intensity(tp, st) : launch_mzcr(tp, st)));
         PROF(o.kind == SOP_ENERGY ? "energy_kernel" : (o.kind == SOP_INTENSITY ? "intensity_kernel" : "mzcr_kernel"));
       }
     }

@@ -25,9 +25,6 @@ constexpr int kFmtWarps = 8;               // warps per CTA = frames per transfo
 constexpr int kFmtThreads = kFmtWarps * 32;
 constexpr int kFmtFpw = 2;                 // frames per warp in the per-frame phase: a half warp each (one lane per lag / root, p <= 15)
 constexpr int kFmtBatch = kFmtWarps * kFmtFpw;
-#ifndef OSM_FMT_BATCHED
-#define OSM_FMT_BATCHED 1
-#endif
 
 struct FmtWarpWs {                          // per-warp scratch of the per-frame phase
   double c[fm::kMaxLpcOrder];               // polynomial, ascending powers (monic)
@@ -39,6 +36,7 @@ struct FmtWarpWs {                          // per-warp scratch of the per-frame
   int n, z0;
 };
 
+template <bool F32>
 __global__ void __launch_bounds__(kFmtThreads) formant_kernel(const FormantParams p)
 {
   extern __shared__ __align__(16) unsigned char fmtSmem[];
@@ -66,7 +64,7 @@ __global__ void __launch_bounds__(kFmtThreads) formant_kernel(const FormantParam
       float *planes = xw;                                        // [kFmtWarps][4][kPlane]: in / out, real / imaginary
       const float *wc = p.D, *cosT = p.D + ro::kNw + ro::kNc, *sinT = cosT + (size_t)p.kHalf * IP;
       for (int f = 0; f < nb; f++) {
-        FrameReader fr{tp, tp.pcm + (uo + (long long)(tl.f0 + fb + f) * tp.frameStep) * tp.nChan};
+        FrameReader<F32> fr{tp, tp.pcm + (uo + (long long)(tl.f0 + fb + f) * tp.frameStep) * tp.nChan};
         float *re = planes + (size_t)f * 4 * ro::kPlane, *im = re + ro::kPlane;
         for (int n = tid; n < ro::kN; n += kFmtThreads) {
           const int m = n - p.padLeft;
@@ -145,7 +143,7 @@ __global__ void __launch_bounds__(kFmtThreads) formant_kernel(const FormantParam
     } else {
     // 1. windowed frames (dspcore/windower.cpp:226) into shared memory
     for (int f = 0; f < nb; f++) {
-      FrameReader fr{tp, tp.pcm + (uo + (long long)(tl.f0 + fb + f) * tp.frameStep) * tp.nChan};
+      FrameReader<F32> fr{tp, tp.pcm + (uo + (long long)(tl.f0 + fb + f) * tp.frameStep) * tp.nChan};
       for (int m = tid; m < N; m += kFmtThreads) xw[f * N + m] = fr.at(m);
     }
     __syncthreads();
@@ -176,8 +174,7 @@ __global__ void __launch_bounds__(kFmtThreads) formant_kernel(const FormantParam
       // The sequential per-frame steps (Durbin recursion, candidate selection / sort / store) run as "one LANE per frame" on the
       // first warp for the whole batch of frames -- one instruction stream for up to 16 frames instead of one per half warp with a
       // single active lane (ncu: those two steps were 45 % of the kernel's warp-instructions) -- the steps with per-frame
-      // parallelism (autocorrelation lags, the simultaneous root refinement) stay "one half warp per frame".  OSM_FMT_BATCHED=0
-      // builds the previous flow for A/B runs.
+      // parallelism (autocorrelation lags, the simultaneous root refinement) stay "one half warp per frame".
       const bool live = fb0 + fi < tl.nf;
       FmtWarpWs &w = ws[live ? fi : 0];
       const int P = p.p;
@@ -211,15 +208,9 @@ __global__ void __launch_bounds__(kFmtThreads) formant_kernel(const FormantParam
         const float *x = res0 + ((size_t)part * kFmtWarps + fin) * IP;
         if (hl <= P) w.r[hl] = fm::acf_lag(x, I, hl);                  // lld/lpc.cpp:156-215 (method acf)
       }
-#if OSM_FMT_BATCHED
       __syncthreads();
       if (warp == 0 && lane < kFmtWarps * fpw && fb0 + lane < tl.nf) lpc_setup(ws[lane]);
       __syncthreads();
-#else
-      __syncwarp(hm);
-      if (live && hl == 0) lpc_setup(w);
-      __syncwarp(hm);
-#endif
       if (live) {
       const int n = w.n;
       const double *c = w.c + w.z0;
@@ -246,15 +237,9 @@ __global__ void __launch_bounds__(kFmtThreads) formant_kernel(const FormantParam
         w.ok[hl] = fm::root_to_formant(zr, zi, p.T, p.minF, p.maxF, &f, &b) ? 1 : 0;
         w.f[hl] = f; w.b[hl] = b;
       }
-#if !OSM_FMT_BATCHED
-      __syncwarp(hm);
-      if (hl == 0) emit(w, fi);
-#endif
       }
-#if OSM_FMT_BATCHED
       __syncthreads();
       if (warp == 0 && lane < kFmtWarps * fpw && fb0 + lane < tl.nf) emit(ws[lane], lane);
-#endif
     }
     __syncthreads();
   }
@@ -272,11 +257,12 @@ cudaError_t launch_formant(const FormantParams &p, cudaStream_t st)
 {
   if (p.tp.nTiles <= 0) return cudaSuccess;
   const size_t smem = formant_smem_bytes(p);
+  auto kern = p.tp.pcmF32 ? formant_kernel<true> : formant_kernel<false>;
   if (smem > 48 * 1024) {   // per device / context attribute: set on every launch like the other launchers
-    cudaError_t e = cudaFuncSetAttribute(formant_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
   }
-  formant_kernel<<<p.tp.nTiles, kFmtThreads, smem, st>>>(p);
+  kern<<<p.tp.nTiles, kFmtThreads, smem, st>>>(p);
   return cudaGetLastError();
 }
 

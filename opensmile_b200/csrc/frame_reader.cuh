@@ -9,9 +9,11 @@ namespace osm {
 // ------------------------------------------------------------------------------------------
 // time-domain frames: sample n of frame t, as the framer (or the windower) level holds it
 // ------------------------------------------------------------------------------------------
+// F32: the kernel instance for pre-converted mono float samples (TimeOpParams::pcmF32)
+template <bool F32>
 __device__ __forceinline__ float td_pcm(const TimeOpParams &p, const int16_t *s)
 {
-  if (OSM_PCM_F32_SUPPORT && p.pcmF32) return *reinterpret_cast<const float *>(s);   // pre-converted mono float sample
+  if constexpr (F32) return *reinterpret_cast<const float *>(s);   // pre-converted mono float sample
   // smileutil/smileUtil.c:2520-2534 : ((sum_c (float)x_c) / nChan) / 32767
   float tmp = (float)s[0];
   for (int c = 1; c < p.nChan; c++) tmp = __fadd_rn(tmp, (float)s[c]);
@@ -26,10 +28,11 @@ __device__ __forceinline__ float td_pcm(const TimeOpParams &p, const int16_t *s)
   return __fdiv_rn(__fdiv_rn(tmp, (float)p.nChan), 32767.0f);
 }
 
+template <bool F32>
 struct FrameReader {
   const TimeOpParams &p;
   const int16_t *base;     // first sample frame of this frame
-  __device__ __forceinline__ float raw(int n) const { return td_pcm(p, base + (long long)n * p.nChan); }
+  __device__ __forceinline__ float raw(int n) const { return td_pcm<F32>(p, base + (long long)n * p.nChan); }
   // the cVectorPreemphasis level (the framer level when p.preemph = 0)
   __device__ __forceinline__ float pre(int n) const
   {

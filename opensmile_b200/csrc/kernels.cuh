@@ -3,60 +3,6 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 
-// The kernels that read PCM (kernels.cu, ops.cu, pitch.cu, formant.cu) are compiled TWICE (Makefile): the default objects read
-// int16 only (OSM_PCM_F32_SUPPORT = 0) -- a run-time "float samples?" test inside the sample accessors made the ComParE step
-// measurably slower, device-resident and end to end -- and the _f32 objects
-// (-DOSM_F32_VARIANT) read the mono float buffer pcm_convert_kernel produces for the other sample formats.  Under OSM_F32_VARIANT every
-// external function of those translation units gets the suffix _f32; api.cu picks launch_*_f32 for plans whose input is not int16.
-#ifdef OSM_F32_VARIANT
-#define OSM_PCM_F32_SUPPORT 1
-#define lld_tile_frames lld_tile_frames_f32
-#define lld_virtual_warps lld_virtual_warps_f32
-#define lld_max_chunk_tiles lld_max_chunk_tiles_f32
-#define lld_supported_fft lld_supported_fft_f32
-#define lld_smem_bytes lld_smem_bytes_f32
-#define launch_lld launch_lld_f32
-#define post_tile_rows post_tile_rows_f32
-#define launch_post launch_post_f32
-#define acf_pitch_supported_fft acf_pitch_supported_fft_f32
-#define launch_acf_pitch launch_acf_pitch_f32
-#define launch_rasta launch_rasta_f32
-#define launch_plp_tail launch_plp_tail_f32
-#define launch_cms_means launch_cms_means_f32
-#define launch_vecop_ll1 launch_vecop_ll1_f32
-#define launch_pitch_smooth launch_pitch_smooth_f32
-#define launch_spectral launch_spectral_f32
-#define launch_mag_rows launch_mag_rows_f32
-#define launch_intensity launch_intensity_f32
-#define launch_energy launch_energy_f32
-#define launch_mzcr launch_mzcr_f32
-#define launch_shs launch_shs_f32
-#define launch_viterbi launch_viterbi_f32
-#define launch_jitter launch_jitter_f32
-#define launch_seq_post launch_seq_post_f32
-#define formant_smem_bytes formant_smem_bytes_f32
-#define launch_formant launch_formant_f32
-#define lpc_smem_bytes lpc_smem_bytes_f32
-#define launch_lpc launch_lpc_f32
-// kernels with external / weak linkage in kernels.cu and ops.cu (the other files keep theirs in anonymous namespaces)
-#define lld_kernel lld_kernel_f32
-#define acf_pitch_kernel acf_pitch_kernel_f32
-#define cms_mean_kernel cms_mean_kernel_f32
-#define energy_kernel energy_kernel_f32
-#define intensity_kernel intensity_kernel_f32
-#define mag_rows_kernel mag_rows_kernel_f32
-#define mzcr_kernel mzcr_kernel_f32
-#define pitch_smooth_kernel pitch_smooth_kernel_f32
-#define plp_tail_kernel plp_tail_kernel_f32
-#define post_kernel post_kernel_f32
-#define rasta_kernel rasta_kernel_f32
-#define spectral_kernel spectral_kernel_f32
-#define vecop_ll1_kernel vecop_ll1_kernel_f32
-#endif
-#ifndef OSM_PCM_F32_SUPPORT
-#define OSM_PCM_F32_SUPPORT 0
-#endif
-
 namespace osm {
 
 constexpr int kMaxVW = 32;   // virtual warps (F-lane groups) per CTA
@@ -81,6 +27,8 @@ struct LldParams {
   int nChan;
   // 1: `pcm` holds pre-converted mono float samples (pcm_convert_kernel: every input format but 16-bit integer).  The sample
   // frame is 4 bytes wide, so nChan is 2 here -- all offset arithmetic stays in int16 units -- and only the conversion differs.
+  // Every kernel that reads PCM has an instance per format (template flag F32); its launcher picks it from this field.  A
+  // run-time "float samples?" test inside the sample accessors made the ComParE step measurably slower.
   int pcmF32;
   // fused temporal stages (static | delta(W1) | delta(W1,W2)); halo = W1 + W2, 0 when not fused
   unsigned hopMagic;             // ceil(2^32 / frameStep): i / frameStep == __umulhi(i, hopMagic) for i * frameStep < 2^32

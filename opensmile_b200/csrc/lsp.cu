@@ -19,6 +19,7 @@ namespace {
 constexpr int kLpcWarps = 8;
 constexpr int kLpcThreads = kLpcWarps * 32;
 
+template <bool F32>
 __global__ void __launch_bounds__(kLpcThreads) lpc_kernel(const LpcParams p)
 {
   extern __shared__ __align__(16) float lpcSmem[];
@@ -30,7 +31,7 @@ __global__ void __launch_bounds__(kLpcThreads) lpc_kernel(const LpcParams p)
   const long long uo = tp.uttOff[tl.utt];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int f = warp; f < tl.nf; f += kLpcWarps) {
-    FrameReader fr{tp, tp.pcm + (uo + (long long)(tl.f0 + f) * tp.frameStep) * tp.nChan};
+    FrameReader<F32> fr{tp, tp.pcm + (uo + (long long)(tl.f0 + f) * tp.frameStep) * tp.nChan};
     for (int n = lane; n < N; n += 32) xs[n] = tp.windowed ? fr.at(n) : fr.pre(n);
     __syncwarp();
     if (lane <= P) rs[f * (P + 1) + lane] = fm::acf_lag(xs, N, lane);
@@ -63,11 +64,12 @@ cudaError_t launch_lpc(const LpcParams &p, cudaStream_t st)
 {
   if (p.tp.nTiles <= 0) return cudaSuccess;
   const size_t smem = lpc_smem_bytes(p);
+  auto kern = p.tp.pcmF32 ? lpc_kernel<true> : lpc_kernel<false>;
   if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(lpc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
   }
-  lpc_kernel<<<p.tp.nTiles, kLpcThreads, smem, st>>>(p);
+  kern<<<p.tp.nTiles, kLpcThreads, smem, st>>>(p);
   return cudaGetLastError();
 }
 

@@ -389,13 +389,14 @@ cudaError_t launch_mag_rows(const float *mag, const OpTile *tiles, int nTiles, i
   return cudaGetLastError();
 }
 
+template <bool F32>
 __global__ void __launch_bounds__(32) energy_kernel(const TimeOpParams p)
 {
   const OpTile tl = p.tiles[blockIdx.x];
   const int lane = threadIdx.x;
   if (lane >= tl.nf) return;
   const long long uo = p.uttOff[tl.utt];
-  FrameReader fr{p, p.pcm + (uo + (long long)(tl.f0 + lane) * p.frameStep) * p.nChan};
+  FrameReader<F32> fr{p, p.pcm + (uo + (long long)(tl.f0 + lane) * p.frameStep) * p.nChan};
   const int N = p.frameSize;
   double d = 0.0;                                     // lldcore/energy.cpp:157-161
   for (int i = 0; i < N; i++) { const float t = fr.at(i); d += (double)__fmul_rn(t, t); }
@@ -416,13 +417,14 @@ __global__ void __launch_bounds__(32) energy_kernel(const TimeOpParams p)
   }
 }
 
+template <bool F32>
 __global__ void __launch_bounds__(32) mzcr_kernel(const TimeOpParams p)
 {
   const OpTile tl = p.tiles[blockIdx.x];
   const int lane = threadIdx.x;
   if (lane >= tl.nf) return;
   const long long uo = p.uttOff[tl.utt];
-  FrameReader fr{p, p.pcm + (uo + (long long)(tl.f0 + lane) * p.frameStep) * p.nChan};
+  FrameReader<F32> fr{p, p.pcm + (uo + (long long)(tl.f0 + lane) * p.frameStep) * p.nChan};
   const int N = p.frameSize;
   float mean = fr.at(0), nzc = 0.0f, nmc = 4.0f, mx = 0.f, mn = 0.f, absmax = 0.f;   // lldcore/mzcr.cpp:113-115
   if (p.zZcr || p.zMcr || p.zDc) {
@@ -462,13 +464,14 @@ __global__ void __launch_bounds__(32) mzcr_kernel(const TimeOpParams p)
 // cIntensity (lldcore/intensity.cpp:124-146).  The reference bounds its summation loop by
 // MIN(Nsrc, MIN(nWin, Ndst)) with Ndst = number of OUTPUT values (1 or 2), i.e. only the first one or
 // two samples of the frame enter the "mean": reproduced as is, this is what the shipped configs emit.
+template <bool F32>
 __global__ void __launch_bounds__(32) intensity_kernel(const TimeOpParams p)
 {
   const OpTile tl = p.tiles[blockIdx.x];
   const int lane = threadIdx.x;
   if (lane >= tl.nf) return;
   const long long uo = p.uttOff[tl.utt];
-  FrameReader fr{p, p.pcm + (uo + (long long)(tl.f0 + lane) * p.frameStep) * p.nChan};
+  FrameReader<F32> fr{p, p.pcm + (uo + (long long)(tl.f0 + lane) * p.frameStep) * p.nChan};
   const int nOut = (p.iIntensity ? 1 : 0) + (p.iLoudness ? 1 : 0);
   const int safeN = min(p.frameSize, nOut);
   double Im = 0.0;
@@ -484,20 +487,20 @@ __global__ void __launch_bounds__(32) intensity_kernel(const TimeOpParams p)
 cudaError_t launch_intensity(const TimeOpParams &p, cudaStream_t st)
 {
   if (p.nTiles <= 0) return cudaSuccess;
-  intensity_kernel<<<p.nTiles, 32, 0, st>>>(p);
+  (p.pcmF32 ? intensity_kernel<true> : intensity_kernel<false>)<<<p.nTiles, 32, 0, st>>>(p);
   return cudaGetLastError();
 }
 
 cudaError_t launch_energy(const TimeOpParams &p, cudaStream_t st)
 {
   if (p.nTiles <= 0) return cudaSuccess;
-  energy_kernel<<<p.nTiles, 32, 0, st>>>(p);
+  (p.pcmF32 ? energy_kernel<true> : energy_kernel<false>)<<<p.nTiles, 32, 0, st>>>(p);
   return cudaGetLastError();
 }
 cudaError_t launch_mzcr(const TimeOpParams &p, cudaStream_t st)
 {
   if (p.nTiles <= 0) return cudaSuccess;
-  mzcr_kernel<<<p.nTiles, 32, 0, st>>>(p);
+  (p.pcmF32 ? mzcr_kernel<true> : mzcr_kernel<false>)<<<p.nTiles, 32, 0, st>>>(p);
   return cudaGetLastError();
 }
 

@@ -1,7 +1,7 @@
 """Static instruction budget of lld512_kernel<13> at the bench geometry (hop 160, frame 400, F = 32, K = 13, 26 bands),
 without a GPU:
 
-    python scripts/lld512_sass_budget.py [-D...]      # extra arguments go to nvcc (e.g. -DOSM_FAST_EMIT_K13=1)
+    python scripts/lld512_sass_budget.py [-D...]      # extra arguments go to nvcc
 
 1. compiles opensmile_b200/csrc/lld_fast.cu for sm_90a (-lineinfo) and disassembles it with inline line information;
 2. gives every instruction of the kernel the lld_fast.cu line it was inlined into and keeps the per-tile loop, split into
