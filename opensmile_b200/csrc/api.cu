@@ -742,7 +742,7 @@ static osm_b200_status build_jitter(const PlanDesc &d, const StaticOp &op, const
   jp.capWav = (int)((capWav + 3) & ~3L);
   jp.capCC = (int)(((long)ceil(2.0 * jo.searchRangeRel * tMax) + 8 + 1) & ~1L);
   jp.capAvg = (int)(((long)ceil(tMax) + 8 + 3) & ~3L);
-  jp.capPb = (int)((capWav / minPer + 8 + 3) & ~3L);
+  jp.capPb = (int)((capWav / minPer + 8 + 3) & ~3L);            // period starts of one frame: toRead / T0min + 2 at most
   if (pc.minPitch < 1.0 || (size_t)4 * ((size_t)jp.capCC * 8 + (size_t)(jp.capWav + jp.capAvg) * 4 + (size_t)jp.capPb * 4) > 200 * 1024)
     return fail(OSM_B200_ERR_UNSUPPORTED, "cPitchJitter: frame size / pitch range need more workspace than the kernel has");
   return OSM_B200_OK;
@@ -1195,6 +1195,17 @@ static osm_b200_status launch_range(osm_b200_plan *pl, const void *d_pcm, float 
       sh.statOff = dS; sh.shs = o.dShs.p;
       CU(launch_shs(sh, ks));
       PROF("shs_kernel");
+      if (d.ops[o.descOp].chain.shsOnly) {
+        // the op's output is the cPitchShs level: its rows (indexed by statOff like dStat) into the op's static columns
+        const long long *hS = pl->hMeta.p + 2 * nm;
+        const long long r0 = hS[u0], nr = hS[u1] - hS[u0];
+        if (nr > 0)
+          CU(cudaMemcpy2DAsync(pl->dStat.p + (size_t)r0 * d.nStatic + d.ops[o.descOp].outCol, (size_t)d.nStatic * sizeof(float),
+                               o.dShs.p + (size_t)r0 * sh.nShsCols, (size_t)sh.nShsCols * sizeof(float), (size_t)sh.nShsCols * sizeof(float),
+                               (size_t)nr, cudaMemcpyDeviceToDevice, ks));
+        pl->lastLaunches++;
+        continue;
+      }
       ViterbiParams vp = o.vit;
       vp.shs = o.dShs.p; vp.uttOff = dU; vp.statOff = dS; vp.stat = pl->dStat.p; vp.lag = o.dLag.p;
       CU(launch_viterbi(vp, u0, u1, ks));
@@ -1387,7 +1398,7 @@ static osm_b200_status run_host_impl(osm_b200_plan *pl, const void *pcm, const i
     CU(cudaMemcpy(&flag, pl->dErr.p, sizeof flag, cudaMemcpyDeviceToHost));
     if (flag) {
       CU(cudaMemset(pl->dErr.p, 0, sizeof(int)));
-      return fail(OSM_B200_ERR_UNSUPPORTED, "cPitchJitter: a frame left the supported geometry (F0 period / read window too long for the kernel's workspace, or a read past the end of the utterance); its rows were zeroed");
+      return fail(OSM_B200_ERR_UNSUPPORTED, "cPitchJitter: a frame left the supported geometry (F0 period / read window too long for the kernel's workspace); its rows were zeroed");
     }
   }
   return OSM_B200_OK;

@@ -430,7 +430,7 @@ struct GraphCompiler {
       case OSM_B200_C_FORMANTLPC: s = build_formant_op(c, op); break;
       case OSM_B200_C_LPC: case OSM_B200_C_LSP: s = build_lpc_op(c, op); break;
       case OSM_B200_C_HARMONICS: s = build_harmonics_op(c, op); break;
-      case OSM_B200_C_VALBASEDSELECTOR: case OSM_B200_C_PITCHSMOOTHERVITERBI: s = build_pitch_chain_op(c, op); break;
+      case OSM_B200_C_VALBASEDSELECTOR: case OSM_B200_C_PITCHSMOOTHERVITERBI: case OSM_B200_C_PITCHSHS: s = build_pitch_chain_op(c, op); break;
       case OSM_B200_C_PITCHJITTER: s = build_jitter_op(c, op); break;
       default: {
         char buf[512];
@@ -844,10 +844,12 @@ struct GraphCompiler {
     return OSM_B200_OK;
   }
 
-  // [cValbasedSelector <-] cPitchSmootherViterbi <- cPitchShs <- cSpecScale <- cFFTmagphase chain
+  // [cValbasedSelector <-] cPitchSmootherViterbi <- cPitchShs <- cSpecScale <- cFFTmagphase chain; c = the cPitchShs itself makes the
+  // op write the cPitchShs level (no Viterbi stage)
   osm_b200_status build_pitch_chain_op(const osm_b200_component *c, StaticOp &op)
   {
     const osm_b200_component *vit = c, *selSrc = nullptr;
+    if (c->type == OSM_B200_C_PITCHSHS) vit = nullptr;
     if (c->type == OSM_B200_C_VALBASEDSELECTOR) {
       const auto &q = c->u.valbasedselector;
       if (c->n_inputs != 2) { err = "cValbasedSelector must read two levels: selector;data"; return OSM_B200_ERR_UNSUPPORTED; }
@@ -856,7 +858,7 @@ struct GraphCompiler {
       vit = R.prod(c->reader_dmLevel[1]);
       if (!selSrc || !vit || vit->type != OSM_B200_C_PITCHSMOOTHERVITERBI) { err = "cValbasedSelector: the data level must come from cPitchSmootherViterbi"; return OSM_B200_ERR_UNSUPPORTED; }
     }
-    const osm_b200_component *shs = single_input(vit);
+    const osm_b200_component *shs = vit ? single_input(vit) : c;
     if (!shs || shs->type != OSM_B200_C_PITCHSHS) { err = "cPitchSmootherViterbi must read a cPitchShs level"; return OSM_B200_ERR_UNSUPPORTED; }
     const osm_b200_component *scl = single_input(shs);
     if (!scl || scl->type != OSM_B200_C_SPECSCALE) { err = "cPitchShs must read a cSpecScale level"; return OSM_B200_ERR_UNSUPPORTED; }
@@ -873,9 +875,20 @@ struct GraphCompiler {
     const FrontEnd &fe = d.streams[op.stream].fe;
     if (selOp >= 0 && !same_geometry(d.streams[d.ops[selOp].stream].fe, fe)) { err = "cValbasedSelector: selector and data levels must share the frame geometry"; return OSM_B200_ERR_UNSUPPORTED; }
     op.kind = SOP_PITCH;
-    if (!build_pitch_chain(scl->u.specscale, shs->u.pitchshs, vit->u.pitchsmootherviterbi, fe.nBins, fe.fftFrameSizeSec, op.chain, err))
+    if (!build_pitch_chain(scl->u.specscale, shs->u.pitchshs, vit ? &vit->u.pitchsmootherviterbi : nullptr, fe.nBins, fe.fftFrameSizeSec,
+                           op.chain, err))
       return OSM_B200_ERR_UNSUPPORTED;
     PitchChainOp &pc = op.chain;
+    if (pc.shsOnly) {                                                 // lldcore/pitchBase.cpp:132-154
+      add_field(op, "nCandidates");
+      add_field(op, "F0Cand", pc.nCand);
+      if (pc.voicing) add_field(op, "candVoicing", pc.nCand);
+      if (pc.scores) add_field(op, "candScores", pc.nCand);
+      const std::pair<bool, const char *> single[] = {{pc.F0C1, "F0C1"}, {pc.voicingC1, "voicingC1"}, {pc.F0raw, "F0raw"}, {pc.voicingClip, "voicingClip"}};
+      for (const auto &o : single) if (o.first) add_field(op, o.second);
+      if (field_elements(op) != pc.nShsCols) { err = "internal: cPitchShs name/element mismatch"; return OSM_B200_ERR_INVALID; }
+      return OSM_B200_OK;
+    }
     if (selOp >= 0) {
       const auto &q = c->u.valbasedselector;
       pc.hasSel = true; pc.selOp = selOp; pc.selThreshold = (float)q.threshold; pc.selOutputVal = (float)q.outputVal;
@@ -901,7 +914,7 @@ struct GraphCompiler {
     int pOp = -1;
     osm_b200_status s2 = get_op(f0c, pOp);
     if (s2 != OSM_B200_OK) return s2;
-    if (d.ops[pOp].kind != SOP_PITCH) { err = "cPitchJitter: the F0 level must come from cPitchSmootherViterbi (optionally through cValbasedSelector)"; return OSM_B200_ERR_UNSUPPORTED; }
+    if (d.ops[pOp].kind != SOP_PITCH || d.ops[pOp].chain.shsOnly) { err = "cPitchJitter: the F0 level must come from cPitchSmootherViterbi (optionally through cValbasedSelector)"; return OSM_B200_ERR_UNSUPPORTED; }
     op.kind = SOP_JITTER;
     op.stream = d.ops[pOp].stream;
     JitterOp &jo = op.jitter;
@@ -949,7 +962,7 @@ struct GraphCompiler {
       osm_b200_status s3 = get_op(sl, so);
       if (s3 != OSM_B200_OK) return s3;
       const StaticOp &po = d.ops[so];
-      if (po.kind != SOP_PITCH) { err = "cValbasedSelector: the selector level must come from the SHS pitch chain (cPitchSmootherViterbi)"; return OSM_B200_ERR_UNSUPPORTED; }
+      if (po.kind != SOP_PITCH || po.chain.shsOnly) { err = "cValbasedSelector: the selector level must come from the SHS pitch chain (cPitchSmootherViterbi)"; return OSM_B200_ERR_UNSUPPORTED; }
       int col = 0;
       if (!find_field(po, [&](const FieldName &f) { return f.n == 1 && (want ? f.name == want : po.nOut == 1); }, col)) {
         err = want ? std::string("cValbasedSelector: selector element '") + want + "' not found in the pitch level" : std::string("cValbasedSelector: the selector level must hold exactly one element"); return OSM_B200_ERR_UNSUPPORTED;
@@ -1012,7 +1025,7 @@ struct GraphCompiler {
         if (!open) {
           OutGroup g;
           g.srcCol = col; g.n = 0; g.stream = op.stream; g.outCol = d.nOut; g.stages = stages;
-          if (op.kind == SOP_PITCH) { g.lagKind = 1; g.lagOp = opIdx; }
+          if (op.kind == SOP_PITCH && !op.chain.shsOnly) { g.lagKind = 1; g.lagOp = opIdx; }   // the cPitchShs level does not lag
           if (op.kind == SOP_JITTER) { g.lagKind = 2; g.lagOp = op.jitter.pitchOp; }
           if (op.kind == SOP_HARMONICS) { g.lagKind = 1; g.lagOp = op.harmonics.pitchOp; }
           if (gateIdx >= 0) {
@@ -1227,6 +1240,7 @@ struct GraphCompiler {
       if (!seg && g.lagKind == 0) continue;
       if (g.lagKind == 0) { err = "cDeltaRegression.onlyInSegments=1 is only supported behind the SHS pitch chain (cPitchSmootherViterbi / cPitchJitter levels)"; return OSM_B200_ERR_UNSUPPORTED; }
       const size_t ns = g.stages.size();
+      if (ns == 0 && !seg && g.limitStreams.empty()) continue;   // a static level itself: every frame, nothing lags behind it
       bool ok = ns >= 1 && ns <= 2 && g.stages[0].kind == ST_SMA && g.stages[0].win == 1;
       if (ok && ns == 2) ok = g.stages[1].kind == ST_DELTA && (g.stages[1].flags & 1) && g.stages[1].win >= 1 && g.stages[1].win <= 4;
       if (!ok) { err = "levels behind cPitchSmootherViterbi / cPitchJitter support cContourSmoother(smaWin=3) optionally followed by cDeltaRegression(onlyInSegments=1) only"; return OSM_B200_ERR_UNSUPPORTED; }

@@ -227,17 +227,26 @@ __global__ void __launch_bounds__(kShsWarps * 32) shs_kernel(const ShsParams p)
     __syncwarp();
     int nCand = 0;
     if (p.greedy) {
-      // the lane's local maxima (positions 1 + lane + 32 k) as a bit mask, found once
-      unsigned long long pk = 0;
+      // the lane's local maxima (positions 1 + lane + 32 k) as a bit mask, found once: word 0 holds k < 64 (positions up to
+      // 2048), word 1 the rest (nPts <= 4096 puts the last candidate position, nPts - 2, at k <= 127)
+      unsigned long long pk0 = 0, pk1 = 0;
       for (int i = 1 + lane, k = 0; i < M - 1; i += 32, k++) {
         const float s = SS[i];
-        if (SS[i - 1] < s && s > SS[i + 1]) pk |= 1ull << k;
+        if (SS[i - 1] < s && s > SS[i + 1]) {
+          if (k < 64) pk0 |= 1ull << k;
+          else pk1 |= 1ull << (k - 64);
+        }
       }
       float lastS = FLT_MAX; int lastI = -1;
       for (int r = 0; r < nC; r++) {
         float bs = -1.0f; int bi = -1;
-        for (unsigned long long m = pk; m; m &= m - 1) {
+        for (unsigned long long m = pk0; m; m &= m - 1) {
           const int i = 1 + lane + 32 * (__ffsll((long long)m) - 1);
+          const float s = SS[i];
+          if ((s < lastS || (s == lastS && i > lastI)) && s > bs) { bs = s; bi = i; }
+        }
+        for (unsigned long long m = pk1; m; m &= m - 1) {
+          const int i = 1 + lane + 32 * (63 + __ffsll((long long)m));
           const float s = SS[i];
           if ((s < lastS || (s == lastS && i > lastI)) && s > bs) { bs = s; bi = i; }
         }
@@ -391,8 +400,11 @@ __global__ void __launch_bounds__(64) viterbi_kernel(const ViterbiParams p, int 
         copy = (!p.selInvert && val > p.selThreshold) || (p.selInvert && val < p.selThreshold) || (p.selAllowEqual && val == p.selThreshold);
       }
       int n = 0;
-      // semitones above 27.5 Hz, float arithmetic like the reference's log(float) overload (:490-500,512-522)
-      auto semitone = [](float f) -> float { return f > 29.136 ? 12.0f * logf(f / 27.5f) / logf(2.0f) : (f > 0.0 ? 1.0f : 0.0f); };
+      // semitones above 27.5 Hz, float arithmetic like the reference's log(float) overload (:490-500,512-522).  CUDA's logf
+      // is 1 ulp off the host's (glibc) logf on ~5 % of F0 values; the rounded double logarithm differs from it on ~0.1 %
+      auto semitone = [](float f) -> float {
+        return f > 29.136 ? 12.0f * (float)log((double)(f / 27.5f)) / (float)log(2.0) : (f > 0.0 ? 1.0f : 0.0f);
+      };
       if (p.oF0final) o[n++] = copy ? f0 : p.selOutputVal;
       if (p.oF0finalLog) o[n++] = copy ? semitone(f0) : p.selOutputVal;
       if (p.oF0finalEnv || p.oF0finalEnvLog) {
@@ -594,10 +606,14 @@ __global__ void __launch_bounds__(kJitWarps * 32, 6) jitter_kernel(const JitterP
       if (toRead > lenF) toRead = lenF;
       if (maxRead > lenF) maxRead = lenF;
     }
-    bool bad = lastIdx + toRead > L || toRead > kJitWav || toRead < 1;
-    if (F0 > 0.0 && (T0maxF - T0minF + 1 > kJitCC || T0f + 1 > kJitAvg || T0minF < 1 || maxRead / T0minF + 4 > kJitPb)) bad = true;
-    if (bad) {               // the reference drops such a frame (:668-673) or leaves the supported geometry: flagged
-      if (lane == 0) { atomicOr(p.errFlag, 1); for (int k = 0; k < nOutCols; k++) o[k] = 0.0f; }
+    // a read window past the end of the input: the reference's getMatrix fails and the frame is dropped from its level
+    // (:668-673).  That happens only in the last frames (lengthSec can round up to frameSize + 1 samples); the plan keeps one
+    // row per frame, so the row is written as zeros and the state moves on as the reference's does
+    const bool pastEnd = lastIdx + toRead > L;
+    bool bad = toRead > kJitWav || toRead < 1;
+    if (F0 > 0.0 && (T0maxF - T0minF + 1 > kJitCC || T0f + 1 > kJitAvg || T0minF < 1 || toRead / T0minF + 4 > kJitPb)) bad = true;
+    if (bad || pastEnd) {    // outside the supported geometry: flagged
+      if (lane == 0) { if (!pastEnd) atomicOr(p.errFlag, 1); for (int k = 0; k < nOutCols; k++) o[k] = 0.0f; }
       lastIdx += toRead0;
       continue;
     }

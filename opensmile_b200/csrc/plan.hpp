@@ -133,6 +133,7 @@ struct PitchChainOp {
   int lfCutBin = -1;
   bool greedy = false, octaveCorr = false, scores = true, voicing = true, F0C1 = false, voicingC1 = false, F0raw = false, voicingClip = false;
   int nShsCols = 0;
+  bool shsOnly = false;                                      // the op is the cPitchShs level itself: no Viterbi stage, nOut = nShsCols
   // --- cPitchSmootherViterbi
   int bufLen = 30;
   bool oF0final = true, oF0finalLog = false, oF0finalEnv = false, oF0finalEnvLog = false, oVClipped = false, oVUnclipped = false;
@@ -282,7 +283,8 @@ bool build_plp(const osm_b200_plp &cfg, const MelBank &mb, double levelPeriod, P
 bool build_spectral(const osm_b200_spectral &cfg, int nSrc, double fftFrameSizeSec, SpectralOp &op, std::string &err);
 void build_energy(const osm_b200_energy &cfg, EnergyOp &op);
 void build_mzcr(const osm_b200_mzcr &cfg, MzcrOp &op);
-bool build_pitch_chain(const osm_b200_specscale &sc, const osm_b200_pitchshs &ps, const osm_b200_pitchsmootherviterbi &vc,
+// vc == nullptr: the op stops at the cPitchShs level (PitchChainOp::shsOnly)
+bool build_pitch_chain(const osm_b200_specscale &sc, const osm_b200_pitchshs &ps, const osm_b200_pitchsmootherviterbi *vc,
                        int nMag, double fftFrameSizeSec, PitchChainOp &op, std::string &err);
 
 // fe = front end of the windower level the chain's cTransformFFT reads; zeroPadSymmetric = that cTransformFFT's switch

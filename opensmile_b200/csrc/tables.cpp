@@ -476,7 +476,7 @@ void build_mzcr(const osm_b200_mzcr &cfg, MzcrOp &op)
 // cSpecScale::dataProcessorCustomFinalise (dsp/specScale.cpp:236-313), cPitchShs::setupNewNames
 // (lld/pitchShs.cpp:160-215), cPitchBase / cPitchSmootherViterbi configuration.  The spline's abscissa
 // terms (smileUtilSpline.c:124-140) are folded into recurrence coefficients, see PitchChainOp.
-bool build_pitch_chain(const osm_b200_specscale &sc, const osm_b200_pitchshs &ps, const osm_b200_pitchsmootherviterbi &vc,
+bool build_pitch_chain(const osm_b200_specscale &sc, const osm_b200_pitchshs &ps, const osm_b200_pitchsmootherviterbi *vcp,
                        int nMag, double fftFrameSizeSec, PitchChainOp &op, std::string &err)
 {
   if (!(sc.scaleOctave && sc.sourceLin && sc.splineInterp)) { err = "cSpecScale: only scale=octave (log base 2), sourceScale=lin, interpMethod=spline are supported"; return false; }
@@ -545,7 +545,8 @@ bool build_pitch_chain(const osm_b200_specscale &sc, const osm_b200_pitchshs &ps
   if (op.nCand > 8) { err = "cPitchShs.nCandidates > 8 is not supported"; return false; }
   op.scores = ps.scores != 0; op.voicing = ps.voicing != 0; op.F0C1 = ps.F0C1 != 0; op.voicingC1 = ps.voicingC1 != 0;
   op.F0raw = ps.F0raw != 0; op.voicingClip = ps.voicingClip != 0;
-  if (!op.voicing) { err = "cPitchShs.voicing=0 below cPitchSmootherViterbi is not supported"; return false; }
+  op.shsOnly = vcp == nullptr;
+  if (!op.voicing && !op.shsOnly) { err = "cPitchShs.voicing=0 below cPitchSmootherViterbi is not supported"; return false; }
   op.voicingCutoff = (float)ps.voicingCutoff;
   op.octaveCorr = ps.octaveCorrection != 0; op.greedy = ps.greedyPeakAlgo != 0;
   op.nHarm = ps.nHarmonics;
@@ -561,7 +562,9 @@ bool build_pitch_chain(const osm_b200_specscale &sc, const osm_b200_pitchshs &ps
   op.lfCutBin = -1;
   if (ps.lfCut > 0.0) op.lfCutBin = (int)((ceil(log(ps.lfCut) / log(base)) - op.Fmint) / op.Fstept);   // :230-236
   op.nShsCols = 1 + op.nCand * (1 + (int)op.voicing + (int)op.scores) + (int)op.F0C1 + (int)op.voicingC1 + (int)op.F0raw + (int)op.voicingClip;
+  if (op.shsOnly) { op.nOut = op.nShsCols; return true; }
   // cPitchSmootherViterbi (lld/pitchSmootherViterbi.cpp:260-292; setWeights stores tvv in wTvvd, hpp:291-299)
+  const osm_b200_pitchsmootherviterbi &vc = *vcp;
   op.bufLen = vc.bufferLength;
   if (op.bufLen < 2 || op.bufLen > 64) { err = "cPitchSmootherViterbi.bufferLength must be 2..64"; return false; }
   if (vc.F0raw || vc.voicingC1 || vc.voicingClip) { err = "cPitchSmootherViterbi: the copied fields F0raw / voicingC1 / voicingClip are not supported"; return false; }
