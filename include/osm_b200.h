@@ -46,7 +46,8 @@ extern "C" {
 
 /* 2: component types cSpecScale .. cPitchJitter appended (existing values and struct layouts unchanged)
  * 3: cSpecResample, cLpc, cFormantLpc, cDataSelector, cHarmonics appended (same rule; sizeof(osm_b200_component) grows);
- *    later cLsp appended under the same number: a new enum value at the end, no struct layout or size changes */
+ *    later cLsp appended under the same number: a new enum value at the end, no struct layout or size changes;
+ *    cTonespec and cChroma likewise (their parameter blocks are smaller than the union) */
 #define OSM_B200_ABI_VERSION 3
 #if defined(__GNUC__)
 #define OSM_B200_API __attribute__((visibility("default")))
@@ -100,6 +101,8 @@ typedef enum {
   OSM_B200_C_DATASELECTOR,       /* cDataSelector       src/core/dataSelector.cpp:296-366 (elementMode=1)    */
   OSM_B200_C_HARMONICS,          /* cHarmonics          src/lld/harmonics.cpp:743-935 (GeMAPS switch set)    */
   OSM_B200_C_LSP,                /* cLsp                src/lld/lsp.cpp:113-313 (on a stand-alone cLpc level) */
+  OSM_B200_C_TONESPEC,           /* cTonespec           src/lld/tonespec.cpp:89-441 (on a cFFTmagphase magnitude level) */
+  OSM_B200_C_CHROMA,             /* cChroma             src/lld/chroma.cpp:46-117 (on a cTonespec level)  */
   OSM_B200_C_COUNT_
 } osm_b200_component_type;
 
@@ -342,6 +345,22 @@ typedef struct {            /* cLsp: reads a cLpc level (its lpcCoeff field) */
   int32_t processArrayFields;   /* 1 (the cVectorProcessor default); only 0 is supported */
 } osm_b200_lsp;
 
+/* cTonespec.filterType (lld/tonespec.cpp:107-111) */
+typedef enum { OSM_B200_TONE_GAU = 0, OSM_B200_TONE_TRI, OSM_B200_TONE_TRP, OSM_B200_TONE_REC } osm_b200_tone_filter;
+
+typedef struct {            /* cTonespec (lld/tonespec.cpp:46-52) */
+  int32_t nOctaves;         /* 6 */
+  double  firstNote;        /* 55 Hz */
+  int32_t filterType;       /* osm_b200_tone_filter, OSM_B200_TONE_GAU */
+  int32_t usePower;         /* 0 */
+  int32_t dbA;              /* 1 */
+} osm_b200_tonespec;
+
+typedef struct {            /* cChroma (lld/chroma.cpp:46-49) */
+  int32_t octaveSize;       /* 12 */
+  double  silThresh;        /* 0.001 */
+} osm_b200_chroma;
+
 /* one `[name:cType]` section */
 typedef struct {
   int32_t type;                                  /* osm_b200_component_type */
@@ -385,6 +404,8 @@ typedef struct {
     osm_b200_dataselector dataselector;
     osm_b200_harmonics harmonics;
     osm_b200_lsp lsp;
+    osm_b200_tonespec tonespec;
+    osm_b200_chroma chroma;
   } u;
 } osm_b200_component;
 
@@ -434,6 +455,14 @@ OSM_B200_API int64_t     osm_b200_plan_num_frames(const osm_b200_plan *plan, int
 /* the window table cWindower multiplies a frame of n samples with (dspcore/windower.cpp:159-217: window function, squareRoot,
  * fade, gain), as float: what osm_b200_plan_create stages for the kernels (bindings, tests) */
 OSM_B200_API osm_b200_status osm_b200_window_table(const osm_b200_windower *cfg, int32_t n, float *out);
+/* the tables cTonespec builds for a magnitude level of n_bins bins and frame length frame_size_sec (after cTransformFFT's
+ * rescale, so 1 / frame_size_sec = fs / N_fft): note frequencies pitch_class_freq[nNotes + 2], bin_key[n_bins] (nearest note of
+ * every bin), bin_count[nNotes + 2] (bins per note over firstBin .. lastBin), filter_map[n_bins] (filter weight times the
+ * shifted dB(A) weight, zero outside firstBin .. lastBin) and fl_bin[2] = firstBin, lastBin (lld/tonespec.cpp:147-367),
+ * as osm_b200_plan_create stages them for the kernels (bindings, tests).  nNotes = 12 * cfg->nOctaves. */
+OSM_B200_API osm_b200_status osm_b200_tone_tables(const osm_b200_tonespec *cfg, int32_t n_bins, double frame_size_sec,
+                                                  float *pitch_class_freq, int32_t *bin_key, int32_t *bin_count,
+                                                  float *filter_map, int32_t *fl_bin);
 OSM_B200_API int64_t     osm_b200_plan_num_frames_first_eoi(const osm_b200_plan *plan, int64_t n_sample_frames);
 /* the same for levels behind the SHS pitch chain, whose length at that moment depends on the data: viterbi_frames = frames the
  * cPitchSmootherViterbi level held when end of input was raised (osm_b200_plan_copy_seq_lag after a run; < 0: not known, the

@@ -22,7 +22,10 @@ OK, ERR_INVALID, ERR_UNSUPPORTED, ERR_CUDA, ERR_NOMEM = range(5)
  C_MELSPEC, C_MFCC, C_PLP, C_SPECTRAL, C_ENERGY, C_MZCR, C_ACF, C_PITCHACF,
  C_DELTAREGRESSION, C_CONTOURSMOOTHER, C_VECTORCONCAT, C_VECTOROPERATION, C_FULLINPUTMEAN, C_INTENSITY,
  C_SPECSCALE, C_PITCHSHS, C_PITCHSMOOTHERVITERBI, C_VALBASEDSELECTOR, C_PITCHJITTER,
- C_SPECRESAMPLE, C_LPC, C_FORMANTLPC, C_DATASELECTOR, C_HARMONICS, C_LSP) = range(31)
+ C_SPECRESAMPLE, C_LPC, C_FORMANTLPC, C_DATASELECTOR, C_HARMONICS, C_LSP, C_TONESPEC, C_CHROMA) = range(33)
+
+# cTonespec.filterType (osm_b200_tone_filter)
+TONE_GAU, TONE_TRI, TONE_TRP, TONE_REC = range(4)
 
 TYPE_BY_NAME = {
     "cWaveSource": C_WAVESOURCE, "cExternalAudioSource": C_WAVESOURCE, "cFramer": C_FRAMER,
@@ -37,6 +40,7 @@ TYPE_BY_NAME = {
     "cValbasedSelector": C_VALBASEDSELECTOR, "cPitchJitter": C_PITCHJITTER,
     "cSpecResample": C_SPECRESAMPLE, "cLpc": C_LPC, "cFormantLpc": C_FORMANTLPC,
     "cDataSelector": C_DATASELECTOR, "cHarmonics": C_HARMONICS, "cLsp": C_LSP,
+    "cTonespec": C_TONESPEC, "cChroma": C_CHROMA,
 }
 
 WIN_BY_NAME = {"rec": 0, "han": 1, "ham": 2, "gau": 3, "sin": 4, "tri": 5, "bar": 6}
@@ -221,6 +225,14 @@ class Lsp(C.Structure):
     _fields_ = [("processArrayFields", i32)]
 
 
+class Tonespec(C.Structure):
+    _fields_ = [("nOctaves", i32), ("firstNote", f64), ("filterType", i32), ("usePower", i32), ("dbA", i32)]
+
+
+class Chroma(C.Structure):
+    _fields_ = [("octaveSize", i32), ("silThresh", f64)]
+
+
 class _U(C.Union):
     _fields_ = [("wavesource", WaveSource), ("framer", Framer),
                 ("vectorpreemphasis", VectorPreemphasis), ("windower", Windower),
@@ -232,7 +244,8 @@ class _U(C.Union):
                 ("specscale", SpecScale), ("pitchshs", PitchShs), ("pitchsmootherviterbi", PitchSmootherViterbi),
                 ("valbasedselector", ValbasedSelector), ("pitchjitter", PitchJitter),
                 ("specresample", SpecResample), ("lpc", Lpc), ("formantlpc", FormantLpc),
-                ("dataselector", DataSelector), ("harmonics", Harmonics), ("lsp", Lsp)]
+                ("dataselector", DataSelector), ("harmonics", Harmonics), ("lsp", Lsp),
+                ("tonespec", Tonespec), ("chroma", Chroma)]
 
 
 class Component(C.Structure):
@@ -252,6 +265,7 @@ UNION_FIELD = {
     C_FULLINPUTMEAN: "fullinputmean", C_INTENSITY: "intensity",
     C_SPECSCALE: "specscale", C_PITCHSHS: "pitchshs", C_PITCHSMOOTHERVITERBI: "pitchsmootherviterbi",
     C_VALBASEDSELECTOR: "valbasedselector", C_PITCHJITTER: "pitchjitter",
+    C_TONESPEC: "tonespec", C_CHROMA: "chroma",
 }
 
 # every symbol include/osm_b200.h declares (tests assert the library exports all of them)
@@ -262,7 +276,7 @@ EXPORTS = [
     "osm_b200_plan_frame_period", "osm_b200_plan_frame_size_samples",
     "osm_b200_plan_frame_step_samples", "osm_b200_plan_fft_size", "osm_b200_plan_num_frames", "osm_b200_plan_num_time_frames",
     "osm_b200_plan_frame_offsets", "osm_b200_plan_run_device", "osm_b200_plan_run_host", "osm_b200_plan_run_host_resident",
-    "osm_b200_window_table", "osm_b200_plan_num_frames_first_eoi", "osm_b200_plan_num_frames_first_eoi_v", "osm_b200_plan_copy_seq_lag",
+    "osm_b200_window_table", "osm_b200_tone_tables", "osm_b200_plan_num_frames_first_eoi", "osm_b200_plan_num_frames_first_eoi_v", "osm_b200_plan_copy_seq_lag",
     # include/osm_b200_functionals.h
     "osm_b200_functionals_defaults", "osm_b200_functionals_create", "osm_b200_functionals_destroy", "osm_b200_functionals_num_values",
     "osm_b200_functionals_num_elements", "osm_b200_functionals_element_name", "osm_b200_functionals_run_device", "osm_b200_functionals_run_device_cols", "osm_b200_summary_assemble_device", "osm_b200_plan_sample_frame_bytes", "osm_b200_device_csv_slot_bytes", "osm_b200_device_format_csv", "osm_b200_device_format_rows",
@@ -350,8 +364,9 @@ def lib():
     if L.osm_b200_sizeof_component() != C.sizeof(Component):
         raise RuntimeError("ABI mismatch: sizeof(osm_b200_component) = %d, ctypes mirror = %d"
                            % (L.osm_b200_sizeof_component(), C.sizeof(Component)))
-    if L.osm_b200_component_defaults(C_LSP, C.byref(Component())) != 0:     # the last component type of this mirror
-        raise RuntimeError("ABI mismatch: the library does not know component type %d (cLsp)" % C_LSP)
+    L.osm_b200_tone_tables.argtypes = [C.POINTER(Tonespec), i32, f64, vp, vp, vp, vp, vp]
+    if L.osm_b200_component_defaults(C_CHROMA, C.byref(Component())) != 0:     # the last component type of this mirror
+        raise RuntimeError("ABI mismatch: the library does not know component type %d (cChroma)" % C_CHROMA)
     _lib = L
     return L
 

@@ -304,6 +304,10 @@ osm_b200_status osm_b200_component_defaults(int32_t type, osm_b200_component *c)
     case OSM_B200_C_LPC: c->u.lpc.p = 8; c->u.lpc.saveLPCoeff = 1; break;                                               // lld/lpc.cpp:33-45
     case OSM_B200_C_LSP: c->u.lsp.processArrayFields = 1; break;                                                       // core/vectorProcessor.cpp:37
     case OSM_B200_C_DATASELECTOR: c->u.dataselector.elementMode = 1; break;                                              // core/dataSelector.cpp:39
+    case OSM_B200_C_TONESPEC:              // lld/tonespec.cpp:46-52
+      c->u.tonespec.nOctaves = 6; c->u.tonespec.firstNote = 55.0; c->u.tonespec.filterType = OSM_B200_TONE_GAU; c->u.tonespec.dbA = 1;
+      break;
+    case OSM_B200_C_CHROMA: c->u.chroma.octaveSize = 12; c->u.chroma.silThresh = 0.001; c->copyInputName = 0; break;   // lld/chroma.cpp:46-49
     case OSM_B200_C_HARMONICS: {           // lld/harmonics.cpp:28-56
       auto &q = c->u.harmonics;
       snprintf(q.f0ElementName, sizeof q.f0ElementName, "%s", "F0final");
@@ -402,17 +406,24 @@ static osm_b200_status build_pass(osm_b200_plan *pl, int si, int opIdx, bool dum
     oSplit = put(split.data(), split.size() * sizeof(float2));
     if (opIdx >= 0) {
       const StaticOp &op = d.ops[opIdx];
-      const bool isPlp = op.kind == SOP_PLP;
-      const MelBank &mb = d.mels[isPlp ? op.plp.melIdx : op.mfcc.melIdx];
+      const bool isPlp = op.kind == SOP_PLP, isTone = op.kind == SOP_TONE;
+      const MelBank &mb = isTone ? op.tone.bank : d.mels[isPlp ? op.plp.melIdx : op.mfcc.melIdx];
       const MfccOp &mf = op.mfcc;
       const PlpOp &po = op.plp;
       if (isPlp && po.doLpToCeps && po.firstCC > 1) return fail(OSM_B200_ERR_UNSUPPORTED, "cPlp: firstCC > 1 is not supported");
-      kp.opKind = isPlp ? 1 : 0;
+      kp.opKind = isTone ? 2 : (isPlp ? 1 : 0);
       kp.nBands = mb.nBands; kp.melUsePower = mb.usePower;
       // without a magnitude dump the kernel keeps 2X (4|X|^2) out of the real-FFT split and the
       // exact factor 1/4 of the power path is folded into the band scale
       kp.melScale = (mb.usePower && !dumps) ? mb.outScale * 0.25f : mb.outScale;
-      if (!isPlp) {
+      if (isTone) {
+        // band phase: mean of the weighted bins per note (division by the bin count, sqrt under usePower); back end: the
+        // tone values themselves or the chroma fold.  The per-note bin counts take the DCT table's place.
+        const ToneOp &to = op.tone;
+        kp.nStat = to.nOut; kp.doLog = 0;
+        kp.dctStride = mb.nBands; kp.dctRows = 1;
+        kp.toneSqrt = to.usePower; kp.chromaOct = to.octaveSize; kp.chromaSilThresh = to.silThresh;
+      } else if (!isPlp) {
         kp.nStat = mf.nMfcc; kp.melfloor = mf.melfloor; kp.logMelfloor = mf.logMelfloor; kp.doLog = mf.doLog;
         kp.dctStride = (mb.nBands + 3) / 4 * 4; kp.dctRows = mf.nMfcc;
       } else {
@@ -429,7 +440,7 @@ static osm_b200_status build_pass(osm_b200_plan *pl, int si, int opIdx, bool dum
         const int nvw = lld_virtual_warps(fe.nfft);
         const int nB = mb.nBands;
         // the 512-point MFCC instance (lld_fast.cu) also adds every finished band into its DCT partial sums (~20 more)
-        const double bandCost = (!isPlp && !dumps && lld_fast_applies(kp, fe.nfft)) ? 70.0 : 50.0;
+        const double bandCost = (!isPlp && !isTone && !dumps && lld_fast_applies(kp, fe.nfft)) ? 70.0 : 50.0;
         auto cost = [&](int bs, int be) -> double {          // bands [bs, be) visit ranges bs..be
           if (be <= bs) return 0.0;
           return 6.0 * (mb.rangeBegin[be + 1] - mb.rangeBegin[bs]) + bandCost * (be - bs) + 12.0;
@@ -450,13 +461,15 @@ static osm_b200_status build_pass(osm_b200_plan *pl, int si, int opIdx, bool dum
         for (int w = nvw + 1; w <= kMaxVW; w++) kp.melSplit[w] = nB;
       }
       std::vector<float> dctPad((size_t)kp.dctRows * kp.dctStride, 0.f);
-      if (!isPlp) {
+      if (isTone) {
+        dctPad = op.tone.divisor;
+      } else if (!isPlp) {
         for (int i = 0; i < mf.nMfcc; i++)
           memcpy(&dctPad[(size_t)i * kp.dctStride], &mf.cosT[(size_t)i * mb.nBands], sizeof(float) * mb.nBands);
       } else {
         memcpy(dctPad.data(), po.cosT.data(), sizeof(float) * po.cosT.size());
       }
-      const std::vector<float> &liftV = isPlp ? po.lift : mf.liftFactor;
+      const std::vector<float> &liftV = isPlp ? po.lift : (isTone ? op.tone.divisor : mf.liftFactor);   // the tone op reads no lifter
       std::vector<float> eqlV = isPlp ? po.eql : std::vector<float>(1, 0.f);
       oCoef = put(mb.coef.data(), mb.coef.size() * sizeof(float));
       oRange = put(mb.rangeBegin.data(), mb.rangeBegin.size() * sizeof(int));
@@ -465,7 +478,7 @@ static osm_b200_status build_pass(osm_b200_plan *pl, int si, int opIdx, bool dum
         std::vector<int> vb(mb.nBands + 2, 0);
         for (int r = 0; r <= mb.nBands; r++) {
           vb[r] = (int)visit.size();
-          for (int n = mb.rangeBegin[r]; n < mb.rangeBegin[r + 1]; n++) visit.push_back(make_float2(mb.coef[n], 1.0f - mb.coef[n]));
+          for (int n = mb.rangeBegin[r]; n < mb.rangeBegin[r + 1]; n++) visit.push_back(make_float2(mb.coef[n], mb.oneTap ? 0.f : 1.0f - mb.coef[n]));
           while (visit.size() % 4) visit.push_back(make_float2(0.f, 0.f));
         }
         vb[mb.nBands + 1] = (int)visit.size();
@@ -872,7 +885,7 @@ try {
 
   for (size_t oi = 0; oi < d.ops.size(); oi++) {
     const StaticOp &op = d.ops[oi];
-    if (op.kind == SOP_MFCC || op.kind == SOP_PLP) continue;      // fused into its stream's lld_kernel
+    if (op.kind == SOP_MFCC || op.kind == SOP_PLP || op.kind == SOP_TONE) continue;      // fused into its stream's lld_kernel
     OpRt rt;
     rt.kind = op.kind; rt.stream = op.stream; rt.descOp = (int)oi;
     StreamRt &srt = pl->st[op.stream];
@@ -1433,6 +1446,23 @@ osm_b200_status osm_b200_window_table(const osm_b200_windower *w, int32_t n, flo
   memcpy(out, t.data(), sizeof(float) * (size_t)n);
   return OSM_B200_OK;
 }
+
+osm_b200_status osm_b200_tone_tables(const osm_b200_tonespec *cfg, int32_t n_bins, double frame_size_sec, float *pitch_class_freq,
+                                     int32_t *bin_key, int32_t *bin_count, float *filter_map, int32_t *fl_bin)
+try {
+  if (!cfg || !pitch_class_freq || !bin_key || !bin_count || !filter_map || !fl_bin || n_bins < 2 || !(frame_size_sec > 0.0))
+    return fail(OSM_B200_ERR_INVALID, "bad argument");
+  if (cfg->nOctaves < 1) return fail(OSM_B200_ERR_INVALID, "cTonespec.nOctaves must be >= 1");
+  ToneTables t;
+  std::string err;
+  if (!build_tone_tables(*cfg, n_bins, frame_size_sec, t, err)) return fail(OSM_B200_ERR_UNSUPPORTED, err);
+  memcpy(pitch_class_freq, t.pitchClassFreq.data(), sizeof(float) * t.pitchClassFreq.size());
+  memcpy(bin_key, t.binKey.data(), sizeof(int32_t) * t.binKey.size());
+  memcpy(bin_count, t.nbins.data(), sizeof(int32_t) * t.nbins.size());
+  memcpy(filter_map, t.filterMap.data(), sizeof(float) * t.filterMap.size());
+  fl_bin[0] = t.firstBin; fl_bin[1] = t.lastBin;
+  return OSM_B200_OK;
+} catch (const std::bad_alloc &) { return fail(OSM_B200_ERR_NOMEM, "out of host memory"); }
 
 int64_t osm_b200_plan_num_frames_first_eoi(const osm_b200_plan *pl, int64_t n) { return pl ? desc_num_frames_first_eoi(pl->d, n) : 0; }
 int64_t osm_b200_plan_num_frames_first_eoi_v(const osm_b200_plan *pl, int64_t n, int64_t v) { return pl ? desc_num_frames_first_eoi(pl->d, n, v) : 0; }

@@ -33,7 +33,8 @@ const char *type_name(int t)
     "cTransformFFT", "cFFTmagphase", "cMelspec", "cMfcc", "cPlp", "cSpectral", "cEnergy",
     "cMZcr", "cAcf", "cPitchACF", "cDeltaRegression", "cContourSmoother", "cVectorConcat",
     "cVectorOperation", "cFullinputMean", "cIntensity", "cSpecScale", "cPitchShs", "cPitchSmootherViterbi",
-    "cValbasedSelector", "cPitchJitter", "cSpecResample", "cLpc", "cFormantLpc", "cDataSelector", "cHarmonics", "cLsp"};
+    "cValbasedSelector", "cPitchJitter", "cSpecResample", "cLpc", "cFormantLpc", "cDataSelector", "cHarmonics", "cLsp",
+    "cTonespec", "cChroma"};
   return (t >= 0 && t < OSM_B200_C_COUNT_) ? names[t] : "?";
 }
 
@@ -47,6 +48,8 @@ const char *default_name_append(int t)
     case OSM_B200_C_CONTOURSMOOTHER: return "sma";
     case OSM_B200_C_ACF: return "acf";
     case OSM_B200_C_ENERGY: return "energy";
+    case OSM_B200_C_TONESPEC: return "note";       // lld/tonespec.cpp:47
+    case OSM_B200_C_CHROMA: return "chroma";       // lld/chroma.cpp:46
     default: return "";
   }
 }
@@ -432,6 +435,7 @@ struct GraphCompiler {
       case OSM_B200_C_HARMONICS: s = build_harmonics_op(c, op); break;
       case OSM_B200_C_VALBASEDSELECTOR: case OSM_B200_C_PITCHSMOOTHERVITERBI: case OSM_B200_C_PITCHSHS: s = build_pitch_chain_op(c, op); break;
       case OSM_B200_C_PITCHJITTER: s = build_jitter_op(c, op); break;
+      case OSM_B200_C_TONESPEC: case OSM_B200_C_CHROMA: s = build_tone_op(c, op); break;
       default: {
         char buf[512];
         snprintf(buf, sizeof buf, "component '%s' (%s) is not a supported static LLD producer", c->name, type_name(c->type));
@@ -944,6 +948,41 @@ struct GraphCompiler {
     return OSM_B200_OK;
   }
 
+  // cTonespec on a plain cFFTmagphase magnitude level, or cChroma on such a cTonespec level (config/chroma/chroma_fft.conf): one
+  // band op of the FFT stream.  Both are cVectorProcessors that keep the frame count of the level they read.
+  osm_b200_status build_tone_op(const osm_b200_component *c, StaticOp &op)
+  {
+    const osm_b200_component *ts = c;
+    if (c->type == OSM_B200_C_CHROMA) {
+      ts = single_input(c);
+      if (!ts || ts->type != OSM_B200_C_TONESPEC) { err = "cChroma must read a cTonespec level"; return OSM_B200_ERR_UNSUPPORTED; }
+    }
+    ChainInfo ci;
+    if (!resolve_mag_chain(single_input(ts), ci)) { err = "cTonespec: " + err; return OSM_B200_ERR_UNSUPPORTED; }
+    osm_b200_status s2 = get_stream(ci, true, op.stream);
+    if (s2 != OSM_B200_OK) return s2;
+    const FrontEnd &fe = d.streams[op.stream].fe;
+    op.kind = SOP_TONE;
+    ToneOp &to = op.tone;
+    if (!build_tone(ts->u.tonespec, fe.nBins, fe.fftFrameSizeSec, to, err)) return OSM_B200_ERR_UNSUPPORTED;
+    // the field is "tone" with nNotes elements, whatever the input field is called (lld/tonespec.cpp:370-377)
+    const std::string toneName = name_append_auto(*ts, "tone", nullptr);
+    if (c->type == OSM_B200_C_TONESPEC) {
+      add_field(op, toneName, to.nNotes);
+      return OSM_B200_OK;
+    }
+    const auto &q = c->u.chroma;
+    // lld/chroma.cpp:94-115: with nNotes not a multiple of octaveSize the reference logs an error and writes rows it never set
+    if (q.octaveSize < 1 || to.nNotes % q.octaveSize != 0) {
+      err = "cChroma.octaveSize must divide the number of cTonespec notes (12 * nOctaves)"; return OSM_B200_ERR_UNSUPPORTED;
+    }
+    to.octaveSize = q.octaveSize;
+    to.silThresh = (float)q.silThresh;                                                     // :71
+    to.nOut = q.octaveSize;
+    add_field(op, name_append_auto(*c, toneName, nullptr), q.octaveSize);                 // :78-81
+    return OSM_B200_OK;
+  }
+
   // ---- cValbasedSelector gates: the selector value must be one column of the SHS pitch level (directly, or through a cDataSelector
   // that picks it: GeMAPSv01b_core.lld.conf.inc:385-391) ----
   osm_b200_status resolve_gates()
@@ -1250,7 +1289,7 @@ struct GraphCompiler {
   }
 
   // ---- execution strategy per stream ----
-  // A stream with exactly one band op (MFCC / PLP) and no other spectral consumer evaluates it
+  // A stream with exactly one band op (MFCC / PLP / tone) and no other spectral consumer evaluates it
   // inside lld_kernel; any other spectral consumer reads the magnitude level from HBM.
   osm_b200_status choose_execution()
   {
@@ -1259,7 +1298,7 @@ struct GraphCompiler {
       d.streams[s].bandOps.clear();
       for (size_t o = 0; o < d.ops.size(); o++) {
         if (d.ops[o].stream != (int)s) continue;
-        if (d.ops[o].kind == SOP_MFCC || d.ops[o].kind == SOP_PLP) d.streams[s].bandOps.push_back((int)o);
+        if (d.ops[o].kind == SOP_MFCC || d.ops[o].kind == SOP_PLP || d.ops[o].kind == SOP_TONE) d.streams[s].bandOps.push_back((int)o);
         if (d.ops[o].kind == SOP_SPECTRAL || d.ops[o].kind == SOP_PITCHACF || d.ops[o].kind == SOP_MAG || d.ops[o].kind == SOP_PITCH || d.ops[o].kind == SOP_HARMONICS) nSpec++;
       }
       const int nBand = (int)d.streams[s].bandOps.size();

@@ -58,7 +58,7 @@ struct LldParams {
   float melScale;
   int melUsePower;
   int melSplit[kMaxVW + 1];      // virtual warp w computes bands [melSplit[w], melSplit[w+1])
-  // ---- static LLD op on the mel bands: 0 = cMfcc (log, DCT-II, lifter), 1 = cPlp, -1 = none ----
+  // ---- static LLD op on the mel bands: 0 = cMfcc (log, DCT-II, lifter), 1 = cPlp, 2 = cTonespec [-> cChroma], -1 = none ----
   int opKind;
   // magnitude level for non-fused consumers (cSpectral ...): tile-major [tile][bin][F] floats, or null
   float *magOut;
@@ -77,6 +77,10 @@ struct LldParams {
   // ---- output ----
   float *out;
   int outStride, outCol;
+  // cTonespec / cChroma (opKind 2, lld/tonespec.cpp:403-434, lld/chroma.cpp:86-117): band = note, dctCos = per-note bin counts,
+  // toneSqrt = usePower; chromaOct > 0 folds the notes into that many chroma values, 0 outputs the notes
+  int toneSqrt, chromaOct;
+  float chromaSilThresh;
 };
 
 // temporal post-processing (cDeltaRegression / cContourSmoother chains)

@@ -372,6 +372,47 @@ __device__ __forceinline__ void plp_backend(const LldParams &p, const float *mel
 }
 
 // ------------------------------------------------------------------------------------------
+// cTonespec (lld/tonespec.cpp:403-434), per note after the band walk: the weighted bin sum over the note's bin count (IEEE
+// division as the reference's dst[i] /= n), 0 for a note without bins, then sqrt under usePower (0 for a negative sum).
+// The walk's products are fused into its sums (the mel phase's rounding, where the reference rounds product and sum
+// separately): on the same magnitudes the rows stay within 2.4e-7 of the column scale of the reference's statement order.
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ float tone_mean(float sum, float nbins, int usePower)
+{
+  float v = nbins > 0.f ? __fdiv_rn(sum, nbins) : 0.f;
+  if (usePower) v = v >= 0.f ? __fsqrt_rn(v) : 0.f;
+  return v;
+}
+
+// The tone op's back end for one tile, lane = frame.  chromaOct == 0: the notes are the output.  Else cChroma
+// (lld/chroma.cpp:86-117): chroma i = float sum over octaves j in ascending order of note j * octaveSize + i; one value below
+// silThresh or a zero double total of the sums gives a zero vector, otherwise every value is divided by (float) total.
+// dst = ring slot base, row stride 2F.
+template <int F, int NVW>
+__device__ __forceinline__ void tone_backend(const LldParams &p, const float *melS, float *dst, int vw, int f)
+{
+  const int K = p.chromaOct;
+  if (K == 0) {
+    for (int i = vw; i < p.nBands; i += NVW) dst[i * (2 * F) + f] = melS[i * F + f];
+    return;
+  }
+  if (vw != 0) return;
+  const int nOct = p.nBands / K;
+  double sum = 0.0;
+  bool sil = false;
+  for (int i = 0; i < K; i++) {
+    float s = 0.f;
+    for (int j = 0; j < nOct; j++) s = __fadd_rn(s, melS[(j * K + i) * F + f]);
+    if (s < p.chromaSilThresh) sil = true;
+    sum = __dadd_rn(sum, (double)s);
+    dst[i * (2 * F) + f] = s;
+  }
+  const bool norm = sum != 0.0 && !sil;
+  const float fsum = (float)sum;
+  for (int i = 0; i < K; i++) dst[i * (2 * F) + f] = norm ? __fdiv_rn(dst[i * (2 * F) + f], fsum) : 0.f;
+}
+
+// ------------------------------------------------------------------------------------------
 // Fused delta / delta-delta emission of one interior tile (deltawin = 2 for both stages, no
 // clamping, all rows before EOI): F output rows = statics | delta | delta-delta -> outS laid out
 // like the global rows.  num = 1*(x[t+1]-x[t-1]) + 2*(x[t+2]-x[t-2]) in the reference's order:

@@ -306,6 +306,7 @@ __global__ void __launch_bounds__(NT, MINB) lld_kernel(const LldParams p)
           }
           if (r == bs) { cur = nxt; continue; }
           float mval = __fmul_rn(cur, p.melScale);
+          if (opKind == 2) mval = tone_mean(mval, sDct[r - 1], p.toneSqrt);       // tonespec.cpp:424-434 (doLog = 0)
           if (p.doLog) mval = (mval < p.melfloor) ? p.logMelfloor : logf(mval);   // mfcc.cpp:239-243 / plp.cpp:434-440
           if (opKind == 1 && p.plpAud) {
             // auditory weighting + loudness compression (plp.cpp:488-510)
@@ -357,8 +358,10 @@ __global__ void __launch_bounds__(NT, MINB) lld_kernel(const LldParams p)
       ring[i * (2 * F) + ringBase + f] = __fmul_rn(a0, sLift[i]);
       if (two) ring[i1 * (2 * F) + ringBase + f] = __fmul_rn(a1, sLift[i1]);
     }
-    } else {
+    } else if (opKind == 1) {
       plp_backend<F, NVW>(p, melS, sDct, sLift, reinterpret_cast<float *>(smem + L.zbuf), ring + ringBase, vw, f);
+    } else {
+      tone_backend<F, NVW>(p, melS, ring + ringBase, vw, f);
     }
     __syncthreads();
 

@@ -24,6 +24,26 @@ struct MelBank {
   std::vector<int> rangeBegin;     // size nBands+2 ; rangeBegin[r+1] = end of range r
   float outScale = 1.f;            // htkcompatible scaling (melspec.cpp:559-569)
   bool usePower = false;
+  bool oneTap = false;             // every bin feeds one band only (cTonespec): the (w, 1-w) pair becomes (w, 0)
+};
+
+// cTonespec (lld/tonespec.cpp:147-367): the reference's tables, and the same bank as a one-tap MelBank for the kernel's band walk
+// (range r = the bins of note r, i.e. of output r-1; coef = filter map times the shifted dB(A) weight)
+struct ToneTables {
+  std::vector<float> pitchClassFreq;   // [nNotes + 2]
+  std::vector<int> binKey;             // [nBins]
+  std::vector<int> nbins;              // [nNotes + 2] bins per note over firstBin .. lastBin
+  std::vector<float> filterMap;        // [nBins]
+  int firstBin = 0, lastBin = 0;
+};
+struct ToneOp {
+  int nNotes = 0;
+  bool usePower = false;
+  int octaveSize = 0;                  // > 0: cChroma behind the tonespec, 0: the tonespec level is the op's output
+  float silThresh = 0.f;
+  MelBank bank;
+  std::vector<float> divisor;          // [nNotes] (float)pitchClassNbins[b + 1], 0 = output 0 (:424-434)
+  int nOut = 0;
 };
 
 struct FrontEnd {
@@ -43,7 +63,7 @@ struct FrontEnd {
   bool zeroPadSymmetric = false;   // phase only; magnitude consumers are unaffected
 };
 
-enum StaticOpKind { SOP_MFCC = 0, SOP_PLP, SOP_MELSPEC, SOP_SPECTRAL, SOP_ENERGY, SOP_MZCR, SOP_PITCHACF, SOP_VECOP, SOP_MAG, SOP_INTENSITY, SOP_PITCH, SOP_JITTER, SOP_FORMANT, SOP_HARMONICS, SOP_LPC };
+enum StaticOpKind { SOP_MFCC = 0, SOP_PLP, SOP_MELSPEC, SOP_SPECTRAL, SOP_ENERGY, SOP_MZCR, SOP_PITCHACF, SOP_VECOP, SOP_MAG, SOP_INTENSITY, SOP_PITCH, SOP_JITTER, SOP_FORMANT, SOP_HARMONICS, SOP_LPC, SOP_TONE };
 
 struct MfccOp {
   int melIdx = 0;
@@ -217,6 +237,7 @@ struct StaticOp {
   FormantOp formant;
   HarmonicsOp harmonics;
   LpcOp lpc;
+  ToneOp tone;
 };
 
 // temporal stage applied to a static column range (cWindowProcessor family)
@@ -282,6 +303,10 @@ void build_mfcc(const osm_b200_mfcc &cfg, int nBands, MfccOp &op);
 bool build_plp(const osm_b200_plp &cfg, const MelBank &mb, double levelPeriod, PlpOp &op, std::string &err);
 bool build_spectral(const osm_b200_spectral &cfg, int nSrc, double fftFrameSizeSec, SpectralOp &op, std::string &err);
 void build_energy(const osm_b200_energy &cfg, EnergyOp &op);
+// cTonespec on a magnitude level of nBins bins, frame length fftFrameSizeSec; false (err set) where the reference's table
+// construction writes past its filter map
+bool build_tone_tables(const osm_b200_tonespec &cfg, int nBins, double fftFrameSizeSec, ToneTables &t, std::string &err);
+bool build_tone(const osm_b200_tonespec &cfg, int nBins, double fftFrameSizeSec, ToneOp &op, std::string &err);
 void build_mzcr(const osm_b200_mzcr &cfg, MzcrOp &op);
 // vc == nullptr: the op stops at the cPitchShs level (PitchChainOp::shsOnly)
 bool build_pitch_chain(const osm_b200_specscale &sc, const osm_b200_pitchshs &ps, const osm_b200_pitchsmootherviterbi *vc,

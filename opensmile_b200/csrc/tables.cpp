@@ -730,4 +730,144 @@ void build_ref_fft_tables(std::vector<float> &wc)
   }
 }
 
+// ---- cTonespec (lld/tonespec.cpp).  The reference is C++: its unqualified pow / log / fabs / ceil / floor / round of a float
+// argument resolve to the float overloads (powf, logf, ...); std:: with float arguments names the same functions here. ----
+
+// computeDBA (dsp/dbA.cpp:110-126): curF accumulates F0 in float; bin 0 gets 10^(-inf) = 0.  The compiler folds the float
+// pow(x, 2) into x * x (an exact rewrite: one rounding), which is not always what powf returns at a rounding tie.
+static void tone_dba(std::vector<float> &x, int n, float F0)
+{
+  x.assign(n, 0.f);
+  float curF = 0.0f;
+  for (int i = 0; i < n; i++) {
+    const float cf2 = curF * curF;
+    float tmp = (float)(pow(12200.0, 2.0) * (cf2 * cf2)) / ((cf2 + (float)pow(20.6, 2.0)) * (cf2 + (float)pow(12200.0, 2.0)));
+    tmp /= (float)(sqrt(cf2 + pow(107.7, 2.0)) * sqrt(cf2 + pow(737.9, 2.0)));
+    x[i] = (float)pow(10.0, ((10.0 * std::log(tmp) + 2.0) / 10.0));
+    curF += F0;
+  }
+}
+
+bool build_tone_tables(const osm_b200_tonespec &cfg, int nBins, double frameSizeSec, ToneTables &t, std::string &err)
+{
+  const int nNotes = cfg.nOctaves * 12;                                                      // :93-95
+  const float firstNote = (float)cfg.firstNote;
+  // setPitchclassFreq (:147-167)
+  t.pitchClassFreq.assign(nNotes + 2, 0.f);
+  const float firstNote0 = firstNote / (float)pow(2.0, 1.0 / 12.0);
+  t.pitchClassFreq[0] = firstNote0;
+  double nn = 0.0;
+  for (int i = 1; i < nNotes + 2; i++) {
+    nn += 1.0;
+    t.pitchClassFreq[i] = firstNote0 * (float)pow(2.0, nn / 12.0);
+  }
+  const float *pcf = t.pitchClassFreq.data();
+  // computeFilters (:171-367), blocksize = nBins
+  const float F0 = (float)(1.0 / frameSizeSec);                                             // :196
+  std::vector<float> db;
+  if (cfg.dbA) tone_dba(db, nBins, F0);
+  int firstBin = (int)ceil((pcf[0] + pcf[1]) / (2.0 * F0));                                 // :203-207
+  int lastBin = (int)floor((pcf[nNotes] + pcf[nNotes + 1]) / (2.0 * F0));
+  if (firstBin < 1) firstBin = 1;
+  if (lastBin >= nBins) lastBin = nBins - 1;
+  t.binKey.assign(nBins, 0);                                                                // :210-227
+  int curNote = 0;
+  for (int i = 0; i < nBins; i++) {
+    if (curNote > nNotes) curNote = nNotes;
+    float distance0 = std::fabs(pcf[curNote] - ((float)i * F0));
+    int note1 = curNote;
+    float distance1 = std::fabs(pcf[++note1] - ((float)i * F0));
+    while (distance0 > distance1) {
+      if (note1 > nNotes) break;
+      distance0 = distance1;
+      distance1 = std::fabs(pcf[++note1] - ((float)i * F0));
+    }
+    curNote = note1 - 1;
+    t.binKey[i] = curNote;
+  }
+  t.nbins.assign(nNotes + 2, 0);                                                            // :254-258
+  for (int i = firstBin; i <= lastBin; i++)
+    if (t.binKey[i] >= 0) t.nbins[t.binKey[i]]++;
+  t.filterMap.assign(nBins, 0.f);                                                           // :268-332
+  if (cfg.filterType != OSM_B200_TONE_REC) {
+    for (int b = 1; b < nNotes - 1; b++) {
+      const float start_freq = (pcf[b - 1] + pcf[b]) / 2.0f;
+      const float end_freq = (pcf[b] + pcf[b + 1]) / 2.0f;
+      const float start_bin = start_freq / F0, end_bin = end_freq / F0;
+      const float middle_bin = pcf[b] / F0;
+      int i_start_bin = (int)std::ceil(start_bin);
+      int i_end_bin = (int)std::floor(end_bin);
+      const int i_middle_bin = (int)std::round(pcf[b] / F0);
+      if (i_start_bin > i_end_bin) continue;
+      if (i_end_bin >= nBins) i_end_bin = nBins - 1;
+      if (i_start_bin >= nBins) i_start_bin = nBins - 1;
+      if (i_start_bin < 1) i_start_bin = 1;
+      if (cfg.filterType == OSM_B200_TONE_TRI || cfg.filterType == OSM_B200_TONE_TRP) {
+        if (i_middle_bin > nBins) {
+          // :301-304 would write bins i_start_bin .. i_middle_bin - 1 past the end of the reference's map
+          err = "cTonespec: a triangular filter of a note above the spectrum (the reference writes past its filter map); lower nOctaves";
+          return false;
+        }
+        for (int i = i_start_bin; i < i_middle_bin; i++) {
+          float &m = t.filterMap[i];
+          m = (1.0f - ((middle_bin - (float)i) / (middle_bin - start_bin)));
+          if (m > 1.0f) m = 2.0f - m;
+        }
+        for (int i = i_middle_bin; i <= i_end_bin; i++) {
+          float &m = t.filterMap[i];
+          m = (1.0f - (((float)i - middle_bin) / (end_bin - middle_bin)));
+          if (m > 1.0f) m = 2.0f - m;
+        }
+      } else {                                                                              // :311-323
+        for (int i = i_start_bin; i <= i_end_bin; i++) {
+          const double dist_val = (double)(end_bin - start_bin);
+          if (dist_val > 0.0) {
+            const double x_val = (double)((double)i - middle_bin);
+            const double delta = dist_val / 15.0;
+            t.filterMap[i] = (float)((10.0 / 4.0) * (1.0 / sqrt(2.0 * M_PI)) * exp(-0.5 * (1.0 / delta) * (1.0 / delta) * pow(x_val, 2.0)));
+          }
+        }
+      }
+    }
+  }
+  if (cfg.filterType == OSM_B200_TONE_TRP)                                                 // :328-332
+    for (int i = 0; i < nBins; i++) t.filterMap[i] *= t.filterMap[i];
+  for (int i = 0; i < firstBin; i++) t.filterMap[i] = 0;                                   // :347-352
+  for (int i = lastBin + 1; i < nBins; i++) t.filterMap[i] = 0;
+  if (cfg.dbA)                                                                             // :354-359: db[] applied from bin firstBin on
+    for (int i = firstBin; i <= lastBin; i++) t.filterMap[i] *= db[i - firstBin];
+  t.firstBin = firstBin; t.lastBin = lastBin;
+  return true;
+}
+
+// the per-frame sum (:418-434) as a one-tap band bank: note k (output k-1) sums the bins firstBin .. lastBin with binKey == k,
+// which are contiguous because binKey never decreases with the bin index
+bool build_tone(const osm_b200_tonespec &cfg, int nBins, double fftFrameSizeSec, ToneOp &op, std::string &err)
+{
+  if (cfg.nOctaves < 1 || cfg.nOctaves > 8) { err = "cTonespec.nOctaves must be in 1..8"; return false; }
+  if (!(cfg.firstNote > 0.0)) { err = "cTonespec.firstNote must be > 0"; return false; }
+  ToneTables t;
+  if (!build_tone_tables(cfg, nBins, fftFrameSizeSec, t, err)) return false;
+  const int nNotes = cfg.nOctaves * 12;
+  op.nNotes = nNotes; op.nOut = nNotes;
+  op.usePower = cfg.usePower != 0;
+  MelBank &mb = op.bank;
+  mb.nBands = nNotes; mb.nBins = nBins; mb.oneTap = true; mb.usePower = op.usePower; mb.outScale = 1.f;
+  mb.coef = t.filterMap;
+  mb.rangeBegin.assign(nNotes + 2, t.firstBin);
+  int i = t.firstBin;
+  for (int r = 0; r <= nNotes; r++) {
+    mb.rangeBegin[r] = i;
+    while (i <= t.lastBin && t.binKey[i] <= r) {
+      if (t.binKey[i] < r) { err = "internal: cTonespec bin keys out of order"; return false; }
+      i++;
+    }
+  }
+  mb.rangeBegin[nNotes + 1] = i;
+  mb.nLo = t.firstBin; mb.nHi = i;
+  op.divisor.assign(nNotes, 0.f);
+  for (int k = 0; k < nNotes; k++) op.divisor[k] = (float)t.nbins[k + 1];
+  return true;
+}
+
 }  // namespace osm

@@ -238,7 +238,16 @@ const TypeInfo kTypes[] = {
   {"cPitchSmootherViterbi", OSM_B200_C_PITCHSMOOTHERVITERBI}, {"cValbasedSelector", OSM_B200_C_VALBASEDSELECTOR},
   {"cPitchJitter", OSM_B200_C_PITCHJITTER}, {"cSpecResample", OSM_B200_C_SPECRESAMPLE}, {"cLpc", OSM_B200_C_LPC},
   {"cFormantLpc", OSM_B200_C_FORMANTLPC}, {"cDataSelector", OSM_B200_C_DATASELECTOR},
-  {"cHarmonics", OSM_B200_C_HARMONICS}, {"cLsp", OSM_B200_C_LSP}};
+  {"cHarmonics", OSM_B200_C_HARMONICS}, {"cLsp", OSM_B200_C_LSP}, {"cTonespec", OSM_B200_C_TONESPEC}, {"cChroma", OSM_B200_C_CHROMA}};
+
+// cTonespec.filterType spellings (lld/tonespec.cpp:107-111); any other value leaves the constructor's Gaussian (:83)
+int tone_filter(const std::string &f)
+{
+  for (const char *s : {"tri", "Tri", "triangular", "Triangular"}) if (f == s) return OSM_B200_TONE_TRI;
+  for (const char *s : {"trp", "TrP", "Trp", "triangular-powered", "Triangular-Powered"}) if (f == s) return OSM_B200_TONE_TRP;
+  for (const char *s : {"rec", "Rec", "rectangular", "Rectangular"}) if (f == s) return OSM_B200_TONE_REC;
+  return OSM_B200_TONE_GAU;
+}
 
 int type_of(const std::string &t)
 {
@@ -617,6 +626,15 @@ bool to_component(const Section &s, osm_b200_component &c, std::string &err)
         SETI("octaveCorrection", q.octaveCorrection)
         break;
       }
+      case OSM_B200_C_TONESPEC: {           // lld/tonespec.cpp:46-56: printBinMap / printFilterMap exist in DEBUG builds only
+        auto &q = c.u.tonespec;
+        SETI("nOctaves", q.nOctaves) SETD("firstNote", q.firstNote) SETI("usePower", q.usePower) SETI("dbA", q.dbA)
+        if (f == "filterType") { q.filterType = tone_filter(v); continue; }
+        break;
+      }
+      case OSM_B200_C_CHROMA:               // lld/chroma.cpp:46-49
+        SETI("octaveSize", c.u.chroma.octaveSize) SETD("silThresh", c.u.chroma.silThresh)
+        break;
       default: break;
     }
     // same behaviour as the reference: an unknown field aborts configuration (configManager.cpp:2599)
