@@ -265,7 +265,8 @@ UNION_FIELD = {
     C_FULLINPUTMEAN: "fullinputmean", C_INTENSITY: "intensity",
     C_SPECSCALE: "specscale", C_PITCHSHS: "pitchshs", C_PITCHSMOOTHERVITERBI: "pitchsmootherviterbi",
     C_VALBASEDSELECTOR: "valbasedselector", C_PITCHJITTER: "pitchjitter",
-    C_TONESPEC: "tonespec", C_CHROMA: "chroma",
+    C_SPECRESAMPLE: "specresample", C_LPC: "lpc", C_FORMANTLPC: "formantlpc", C_DATASELECTOR: "dataselector",
+    C_HARMONICS: "harmonics", C_LSP: "lsp", C_TONESPEC: "tonespec", C_CHROMA: "chroma",
 }
 
 # every symbol include/osm_b200.h declares (tests assert the library exports all of them)

@@ -806,7 +806,7 @@ static osm_b200_status build_time_op(const PlanDesc &d, const StaticOp &op, cons
     fp.T = fo.T; fp.minF = fo.minF; fp.maxF = fo.maxF;
     fp.refOrder = fo.refOrder ? 1 : 0; fp.kHalf = fo.kHalf; fp.padLeft = fo.padLeft; fp.halfK = fo.halfK;
     fp.saveFormants = fo.saveFormants; fp.saveBandwidths = fo.saveBandwidths; fp.saveNValid = fo.saveNValid;
-    if (formant_smem_bytes(fp) > 200 * 1024) return fail(OSM_B200_ERR_UNSUPPORTED, "cSpecResample: frame too long for the formant kernel");
+    // the shared-memory limit of formant_kernel is refused by the graph pass (tables.cpp build_formant)
   } else if (op.kind == SOP_LPC) {
     LpcParams &lp = rt.lpc;
     memset(&lp, 0, sizeof lp);

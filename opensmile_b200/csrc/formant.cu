@@ -21,20 +21,11 @@ namespace osm {
 
 namespace {
 
-constexpr int kFmtWarps = 8;               // warps per CTA = frames per transform / resampling batch
+using fm::kFmtWarps;                       // CTA shape and scratch: formant_math.cuh (the graph pass sizes the shared memory)
+using fm::kFmtFpw;
+using fm::kFmtBatch;
+using fm::FmtWarpWs;
 constexpr int kFmtThreads = kFmtWarps * 32;
-constexpr int kFmtFpw = 2;                 // frames per warp in the per-frame phase: a half warp each (one lane per lag / root, p <= 15)
-constexpr int kFmtBatch = kFmtWarps * kFmtFpw;
-
-struct FmtWarpWs {                          // per-warp scratch of the per-frame phase
-  double c[fm::kMaxLpcOrder];               // polynomial, ascending powers (monic)
-  double zr[fm::kMaxLpcOrder], zi[fm::kMaxLpcOrder];
-  double f[fm::kMaxLpcOrder], b[fm::kMaxLpcOrder];
-  float r[fm::kMaxLpcOrder + 1];
-  float a[fm::kMaxLpcOrder];
-  int ok[fm::kMaxLpcOrder];
-  int n, z0;
-};
 
 template <bool F32>
 __global__ void __launch_bounds__(kFmtThreads) formant_kernel(const FormantParams p)
@@ -249,8 +240,7 @@ __global__ void __launch_bounds__(kFmtThreads) formant_kernel(const FormantParam
 
 size_t formant_smem_bytes(const FormantParams &p)
 {
-  const size_t perFrame = p.refOrder ? (size_t)4 * ro::kPlane : (size_t)p.tp.frameSize;
-  return sizeof(FmtWarpWs) * kFmtBatch + ((size_t)kFmtWarps * perFrame + (size_t)kFmtBatch * p.nResPad) * sizeof(float);
+  return fm::formant_smem_bytes(p.refOrder != 0, p.tp.frameSize, p.nResPad);
 }
 
 cudaError_t launch_formant(const FormantParams &p, cudaStream_t st)

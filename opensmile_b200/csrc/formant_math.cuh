@@ -5,6 +5,8 @@
 // the float recursions below follow the reference's statement order.
 #pragma once
 #include <math.h>
+#include <stddef.h>
+#include "fft_ref_order.cuh"
 
 #ifdef __CUDACC__
 #define OSM_FM_HD __host__ __device__ __forceinline__
@@ -17,6 +19,31 @@ namespace fm {
 
 constexpr int kMaxLpcOrder = 16;     // predictor order p (GeMAPS: 11)
 constexpr int kAberthMaxIter = 64;
+
+// CTA shape and per-warp scratch of formant_kernel (formant.cu).  They live here so that the graph pass can size the
+// kernel's shared memory on the host (tables.cpp build_formant) and refuse a geometry before a plan touches a device.
+constexpr int kFmtWarps = 8;               // warps per CTA = frames per transform / resampling batch
+constexpr int kFmtFpw = 2;                 // frames per warp in the per-frame phase: a half warp each (one lane per lag / root, p <= 15)
+constexpr int kFmtBatch = kFmtWarps * kFmtFpw;
+constexpr size_t kFmtSmemLimit = 200 * 1024;
+
+struct FmtWarpWs {                          // per-warp scratch of the per-frame phase
+  double c[kMaxLpcOrder];                   // polynomial, ascending powers (monic)
+  double zr[kMaxLpcOrder], zi[kMaxLpcOrder];
+  double f[kMaxLpcOrder], b[kMaxLpcOrder];
+  float r[kMaxLpcOrder + 1];
+  float a[kMaxLpcOrder];
+  int ok[kMaxLpcOrder];
+  int n, z0;
+};
+
+// dynamic shared memory of formant_kernel: scratch | windowed frames or FFT planes of one batch | resampled frames of
+// kFmtBatch frames
+inline size_t formant_smem_bytes(bool refOrder, int frameSize, int nResPad)
+{
+  const size_t perFrame = refOrder ? (size_t)4 * ro::kPlane : (size_t)frameSize;
+  return sizeof(FmtWarpWs) * kFmtBatch + ((size_t)kFmtWarps * perFrame + (size_t)kFmtBatch * nResPad) * sizeof(float);
+}
 
 // smileDsp_autoCorr (smileutil/smileUtil.c:1560-1569): one lag, float accumulation over i = lag .. n-1
 OSM_FM_HD float acf_lag(const float *x, int n, int lag)

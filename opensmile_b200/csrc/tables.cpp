@@ -10,6 +10,7 @@
 #include <cstring>
 
 #include "plan.hpp"
+#include "formant_math.cuh"
 
 #ifndef M_PI
 #define M_PI 3.14159265358979323846
@@ -630,7 +631,11 @@ bool build_formant(const osm_b200_specresample &rs, const osm_b200_lpc &lp, cons
   const int pad = zeroPadSymmetric ? (K - N) / 2 : 0;
   op.nIn = N; op.nRes = I; op.nResPad = (I + 31) / 32 * 32;
   const double twoPi = 2.0 * M_PI, scale = 1.0 / (double)(K / 2);
-  if (K == 512 && I < K && !getenv("OSM_B200_FORMANT_COMPOSED")) {
+  const bool refOrder = K == 512 && I < K && !getenv("OSM_B200_FORMANT_COMPOSED");
+  // formant_kernel keeps a batch of frames and their resampled copies in shared memory: refused here, while the graph is
+  // compiled, so that a description-only plan refuses what a device plan would
+  if (fm::formant_smem_bytes(refOrder, N, op.nResPad) > fm::kFmtSmemLimit) { err = "cSpecResample: frame too long for the formant kernel"; return false; }
+  if (refOrder) {
     // Reference-order path: the spectrum is computed with the reference's own rounding sequence (fft_ref_order.cuh) and the
     // inverse sum runs over the reference's float tables in its order (smileDsp_initIrdft / smileDsp_irdft,
     // smileutil/smileUtil.c:1752-1820): cos / sin of (2 pi (k i)) / nd evaluated in double, stored as float.

@@ -39,6 +39,8 @@ def _comp(ctype, name, reader, writer, **fields):
             if isinstance(v, str):
                 v = v.encode()
             setattr(u, k, v)
+    elif fields:
+        raise AttributeError("component type %d takes no options, got %s" % (ctype, sorted(fields)))
     return c
 
 

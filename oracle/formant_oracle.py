@@ -199,6 +199,51 @@ def formants_from_lpc(a, T, n_formants, min_f, max_f):
     return freq.astype(f32), bw.astype(f32)
 
 
+def autocorr_rows(X, lags):
+    """autocorr of every row of X [T, n] (the same float accumulation order per row, rows vectorised)"""
+    X = np.asarray(X, f32)
+    T, n = X.shape
+    out = np.zeros((T, lags), f32)
+    for lag in range(lags):
+        prod = (X[:, lag:] * X[:, :n - lag]).astype(f32)
+        acc = np.zeros(T, f32)
+        for i in range(prod.shape[1]):
+            acc = (acc + prod[:, i]).astype(f32)
+        out[:, lag] = acc
+    return out
+
+
+def formant_levels(res, base_period, p, n_formants, min_f, max_f, save_nvalid=0, save_formants=1, save_bandwidths=1):
+    """cLpc (acf, order p) + cFormantLpc on resampled frames res [T, I] -> (rows [T, nOut], lpc [T, p]).
+    nFormants as lld/formantLpc.cpp:160-167 resolves it (above p - 1 or <= 0: p - 1); rows = [nValid] | freq[nF] | bw[nF]
+    (:376-392), nValid = the candidates found before the slots ran out"""
+    nF = n_formants if 0 < n_formants <= p - 1 else p - 1
+    R = autocorr_rows(res, p + 1) if len(res) else np.zeros((0, p + 1), f32)
+    n_out = int(bool(save_nvalid)) + (nF if save_formants else 0) + (nF if save_bandwidths else 0)
+    rows = np.zeros((len(res), n_out), f32)
+    lpcs = np.zeros((len(res), p), f32)
+    for t in range(len(res)):
+        a, _ = lpc_acf(R[t], p)
+        lpcs[t] = a
+        f, b = formants_from_lpc(a, base_period, nF, min_f, max_f)
+        row = ([f32(np.count_nonzero(f))] if save_nvalid else []) + (list(f) if save_formants else []) + (list(b) if save_bandwidths else [])
+        rows[t] = row
+    return rows, lpcs
+
+
+def formant_chain(pcm, sample_rate, frame, step, win, zero_pad_symmetric, target_fs, p, n_formants, min_f, max_f, save_nvalid=0,
+                  save_formants=1, save_bandwidths=1, n_chan=1, exact_fft=False, taps=False):
+    """cFramer -> cWindower -> cTransformFFT -> cSpecResample (target_fs) -> cLpc (p) -> cFormantLpc from int16 PCM, any geometry
+    and option set; exact_fft: the reference's own FFT (needs oracle/_ref/libfftsg.so).  taps: also (res, lpc, base period)"""
+    fe = oracle.frontend(float(sample_rate), frame, step, win=win, zero_pad_symmetric=zero_pad_symmetric)
+    spec = fft_frames_exact(pcm, fe, n_chan) if exact_fft else fft_frames(pcm, fe, n_chan)
+    N, H, nfft, T = oracle.geometry(fe, len(pcm) // n_chan)
+    rs = SpecResample(nfft, float(sample_rate), target_fs, oracle.lib().osm_or_fft_frame_size_sec(C.byref(fe)), frame)
+    res = np.stack([rs(a) for a in spec]) if T > 0 else np.zeros((0, rs.I), f32)
+    rows, lpcs = formant_levels(res, rs.base_period_out, p, n_formants, min_f, max_f, save_nvalid, save_formants, save_bandwidths)
+    return (rows, res, lpcs, rs.base_period_out) if taps else rows
+
+
 def gemaps_formant_chain(pcm, sample_rate=16000.0, taps=False, exact_fft=False, v01a=False):
     """config/gemaps/v01b/GeMAPSv01b_core.lld.conf.inc:43-58,250-286 -> [T, 10] = formantFreqLpc[1..5] | formantBandwidthLpc[1..5];
     exact_fft: the FFT level through the reference's own FFT (bit-identical front end, needs oracle/_ref/libfftsg.so)"""
@@ -311,9 +356,7 @@ def find_harmonics(pitch, mag, frq, n_harm):
         log_rel = False
     else:
         m0 = f32(np.log10(m0))                   # float magnitudeF0 = log10(float)
-        H[0]["lr"] = f32(0.0)
-    if log_rel is False:
-        pass
+    H[0]["lr"] = f32(0.0)                        # also when the fundamental has no magnitude (:560)
     for i in range(1, n_harm):
         if log_rel:
             if H[i]["magi"] > 0.0:
@@ -379,6 +422,91 @@ def _closest_peak(x, idx):
     if x[0] > x[idx] and x[N - 1] > x[idx]:
         return 0 if idx < N // 2 else N - 1
     return idx
+
+
+def parse_harmonic_differences(diffs, have_formants):
+    """harmonicDifferences (lld/harmonics.cpp:84-160): "H<i>" = harmonic i (H0 the fundamental), "A<k>" = the strongest harmonic
+    near formant k, "A0" = the fundamental -> (h1formant, h1idx, h2formant, h2idx) per difference, and the highest harmonic
+    named.  Differences that name a formant are dropped, all of them, when there is no formant level (:296-300)"""
+    out, top, formant = [], 0, False
+    for d in diffs:
+        parts = []
+        for t in d.split("-"):
+            k = int(t[1:])
+            if t[0] == "H":
+                parts += [-1, k]
+                top = max(top, k)
+            elif k == 0:
+                parts += [-1, 0]
+            else:
+                parts += [k, -1]
+                formant = True
+        out.append(tuple(parts))
+    if formant and not have_formants:
+        out = []
+    return out, top
+
+
+def harmonics_row(F0, formant_freq, mag, frq, n_harmonics=100, diffs=("H1-H2", "H1-A3"), fa_start=1, fa_end=3, floor_unvoiced=-201.0,
+                  hnr=True, taps=False):
+    """cHarmonics::processVector for log-relative outputs (lld/harmonics.cpp:743-900): [HNRdBACF if hnr] | differences |
+    formant amplitudes fa_start..fa_end (fa_end = -1: every formant; none without formants or when fa_end < fa_start).
+    nHarmonics is raised to one above the highest harmonic a difference names (:212-217).  formant_freq = None: no formant
+    level.  taps: also the ACF and its chosen lag (the HNR decision)"""
+    have = formant_freq is not None
+    fmt = list(formant_freq) if have else []
+    d, top = parse_harmonic_differences(diffs, have)
+    n_harm = max(n_harmonics, top + 1)
+    if have:
+        end = len(fmt) if fa_end == -1 else min(fa_end, len(fmt))
+        fa_range = range(fa_start, end + 1)
+    else:
+        fa_range = range(0)
+    out = []
+    acf, lag = None, 0
+    if hnr:
+        v, acf, lag = _acf_hnr_tap(mag, F0, frq)
+        out.append(v)
+    if F0 > 0.0:
+        H = find_harmonics(F0, mag, frq, n_harm)
+        fa = []
+        for f in fmt:
+            lo, hi = f32(0.8) * f32(f), f32(1.2) * f32(f)
+            best, bm = -1, f32(0.0)
+            for h, hh in enumerate(H):
+                if lo <= hh["fi"] <= hi and hh["mag"] > bm:
+                    best, bm = h, hh["mag"]
+            fa.append(best)
+        for (h1f, h1i, h2f, h2i) in d:
+            if h1f > 0:
+                h1i = fa[h1f - 1] if h1f <= len(fa) else -1
+            if h2f > 0:
+                h2i = fa[h2f - 1] if h2f <= len(fa) else -1
+            ok1, ok2 = 0 <= h1i < n_harm, 0 <= h2i < n_harm
+            if ok1 and ok2:
+                v = f32(H[h1i]["lr"] - H[h2i]["lr"])
+            elif ok1:
+                v = f32(H[h1i]["lr"] - f32(201.0))
+            elif ok2:
+                v = f32(-201.0 - np.float64(H[h2i]["lr"]))
+            else:
+                out.append(f32(0.0))
+                continue
+            out.append(f32(min(max(v, f32(-201.0)), f32(201.0))))
+        for k in fa_range:
+            out.append(H[fa[k - 1]]["lr"] if 1 <= k <= len(fa) and fa[k - 1] >= 0 else f32(0.0))
+    else:
+        out += [f32(0.0)] * len(d) + [f32(floor_unvoiced)] * len(fa_range)
+    row = np.array(out, f32)
+    return (row, acf, lag) if taps else row
+
+
+def _acf_hnr_tap(mag, F0, frq):
+    """acf_hnr_db with the chosen lag"""
+    v, acf = acf_hnr_db(mag, F0, frq)
+    fs = frq[-1] * 2.0
+    f0bin = int(np.floor(fs / f32(F0))) if F0 > 0.0 else 0
+    return v, acf, (_closest_peak(acf, f0bin) if 0 < f0bin < len(acf) else 0)
 
 
 def harmonics_gemaps(F0, formant_freq, mag, frq, n_harm=100, floor_unvoiced=-201.0):

@@ -70,26 +70,15 @@ int fmh_formants(const float *a, int p, double T, int nF, double minF, double ma
 // ---- the product's table builder (opensmile_b200/csrc/tables.cpp, linked into this harness) + the kernel's
 // resampling loop: xw[T][N] windowed frames -> res[T][I] (fmaf in sample order, as formant_kernel phase 2) ----
 #include <cmath>
+#include <cstdlib>
 #include <string>
 #include "../../opensmile_b200/csrc/plan.hpp"
 
-extern "C" {
-
-// returns I (resampled samples per frame) or -1; *Tper = base period of the cLpc level; res may be null (query)
-int fmh_resample(double sampleRate, int N, int nfft, double frameSizeSec, int zeroPadSymmetric, double targetFs,
-                 int p, int nFormants, const float *xw, int T, float *res, double *Tper)
+namespace {
+// the kernel's resampling of T windowed frames xw[T][N] -> res[T][nRes] with the op's table
+void resample_frames(const osm::FormantOp &op, int N, const float *xw, int T, float *res)
 {
-  osm::FrontEnd fe;
-  fe.sampleRate = sampleRate; fe.frameSize = N; fe.nfft = nfft; fe.frameSizeSec = frameSizeSec;
-  fe.fftFrameSizeSec = frameSizeSec * (double)nfft / (double)N;
-  osm_b200_specresample rs{targetFs, -1.0};
-  osm_b200_lpc lp{}; lp.p = p; lp.saveLPCoeff = 1;
-  osm_b200_formantlpc fl{}; fl.nFormants = nFormants; fl.saveFormants = 1; fl.saveBandwidths = 1; fl.minF = 50; fl.maxF = 5450;
-  osm::FormantOp op;
-  std::string err;
-  if (!osm::build_formant(rs, lp, fl, fe, zeroPadSymmetric != 0, op, err)) return -1;
-  if (Tper) *Tper = op.T;
-  if (res && op.refOrder) {
+  if (op.refOrder) {
     // the kernel's reference-order path (formant.cu): 512-point transform of the zero padded frame, then the float inverse sum
     using namespace osm::ro;
     const float *wc = op.D.data(), *cosT = wc + kNw + kNc, *sinT = cosT + (size_t)op.kHalf * op.nResPad;
@@ -114,15 +103,74 @@ int fmh_resample(double sampleRate, int N, int nfft, double frameSizeSec, int ze
         res[(size_t)t * op.nRes + i] = acc / op.halfK;
       }
     }
-  } else if (res)
+  } else
     for (int t = 0; t < T; t++)
       for (int i = 0; i < op.nRes; i++) {
         float acc = 0.0f;
         for (int m = 0; m < N; m++) acc = fmaf(xw[(size_t)t * N + m], op.D[(size_t)m * op.nResPad + i], acc);
         res[(size_t)t * op.nRes + i] = acc;
       }
+}
+
+// the formant op the graph pass builds for these options (tables.cpp build_formant); false where it refuses them
+bool formant_op(double sampleRate, int N, int nfft, double frameSizeSec, int zeroPadSymmetric, double targetFs, int p, int nFormants,
+                double minF, double maxF, int saveNValid, int saveFormants, int saveBandwidths, osm::FormantOp &op)
+{
+  osm::FrontEnd fe;
+  fe.sampleRate = sampleRate; fe.frameSize = N; fe.nfft = nfft; fe.frameSizeSec = frameSizeSec;
+  fe.fftFrameSizeSec = nfft != N ? frameSizeSec * (double)nfft / (double)N : frameSizeSec;     // graph.cpp, cTransformFFT
+  osm_b200_specresample rs{targetFs, -1.0};
+  osm_b200_lpc lp{}; lp.p = p; lp.saveLPCoeff = 1;
+  osm_b200_formantlpc fl{}; fl.nFormants = nFormants; fl.saveFormants = saveFormants; fl.saveBandwidths = saveBandwidths;
+  fl.saveNumberOfValidFormants = saveNValid; fl.minF = minF; fl.maxF = maxF;
+  // the composed table of a long frame takes seconds to build: the last op is kept for the calls of one case
+  static std::vector<double> lastKey;
+  static osm::FormantOp lastOp;
+  static bool lastOk = false;
+  const std::vector<double> key{sampleRate, (double)N, (double)nfft, frameSizeSec, (double)zeroPadSymmetric, targetFs, (double)p,
+                                (double)nFormants, minF, maxF, (double)saveNValid, (double)saveFormants, (double)saveBandwidths,
+                                getenv("OSM_B200_FORMANT_COMPOSED") ? 1.0 : 0.0};
+  if (key != lastKey) {
+    std::string err;
+    lastOp = osm::FormantOp();                     // build_formant sets the reference-order fields only on that path
+    lastOk = osm::build_formant(rs, lp, fl, fe, zeroPadSymmetric != 0, lastOp, err);
+    lastKey = key;
+  }
+  op = lastOp;
+  return lastOk;
+}
+}  // namespace
+
+extern "C" {
+
+// returns I (resampled samples per frame) or -1; *Tper = base period of the cLpc level; res may be null (query)
+int fmh_resample(double sampleRate, int N, int nfft, double frameSizeSec, int zeroPadSymmetric, double targetFs,
+                 int p, int nFormants, const float *xw, int T, float *res, double *Tper)
+{
+  osm::FormantOp op;
+  if (!formant_op(sampleRate, N, nfft, frameSizeSec, zeroPadSymmetric, targetFs, p, nFormants, 50.0, 5450.0, 0, 1, 1, op)) return -1;
+  if (Tper) *Tper = op.T;
+  if (res) resample_frames(op, N, xw, T, res);
   return op.nRes;
 }
+
+// the path formant_kernel takes for these options: info = {refOrder, gathered (reference order: the inverse sum reads the
+// bins gathered per frame batch), kHalf, padLeft, nRes, nResPad, frames per warp, shared memory bytes}; -1 = refused
+int fmh_formant_path(double sampleRate, int N, int nfft, double frameSizeSec, int zeroPadSymmetric, double targetFs, int p,
+                     int nFormants, int *info)
+{
+  osm::FormantOp op;
+  if (!formant_op(sampleRate, N, nfft, frameSizeSec, zeroPadSymmetric, targetFs, p, nFormants, 50.0, 5450.0, 0, 1, 1, op)) return -1;
+  info[0] = op.refOrder; info[1] = op.refOrder && op.kHalf <= 4 * ((2 * osm::ro::kPlane) / 16);    // formant.cu `gathered`
+  info[2] = op.kHalf; info[3] = op.padLeft; info[4] = op.nRes; info[5] = op.nResPad;
+  info[6] = (op.p + 1 <= 16) ? osm::fm::kFmtFpw : 1;                                               // formant.cu `fpw`
+  info[7] = (int)osm::fm::formant_smem_bytes(op.refOrder, N, op.nResPad);
+  return 0;
+}
+
+// formant_kernel's shared memory (formant_math.cuh) and the limit above which the graph pass refuses an op
+long fmh_formant_smem(int refOrder, int N, int nResPad) { return (long)osm::fm::formant_smem_bytes(refOrder != 0, N, nResPad); }
+long fmh_formant_smem_limit() { return (long)osm::fm::kFmtSmemLimit; }
 
 }
 
@@ -175,6 +223,70 @@ int fmh_harmonics(float F0, const float *formants, int nFmt, const float *mag, i
     for (int k = faStart; k <= faEnd; k++) out[o++] = floorUnvoiced;
   }
   return o;
+}
+
+// fmh_harmonics over T rows: F0[T], formants[T][nFmt], mag[T][nb] -> out[T][nOut]; returns nOut
+int fmh_harmonics_rows(int T, const float *F0, const float *formants, int nFmt, const float *mag, int nb, double binHz, int nHarm,
+                       int nDiffs, const int *diffs, int faStart, int faEnd, float floorUnvoiced, int doHnr, float *out)
+{
+  const int nOut = (doHnr ? 1 : 0) + nDiffs + (faEnd >= faStart ? faEnd - faStart + 1 : 0);
+  for (int t = 0; t < T; t++)
+    fmh_harmonics(F0[t], formants + (size_t)t * nFmt, nFmt, mag + (size_t)t * nb, nb, binHz, nHarm, nDiffs, diffs, faStart, faEnd,
+                  floorUnvoiced, doHnr, out + (size_t)t * nOut);
+  return nOut;
+}
+
+// harmonics_kernel's per-lane shortcut: lane i takes its predecessor's candidate bin from the closed form freq_to_bin(i F0, 0)
+// and checks that its own candidate equals freq_to_bin((i + 1) F0, 0).  Returns the first harmonic whose check fails (the
+// kernel then falls back to the sequential search), -1 if every check holds.  The candidates depend on F0 and the axis only.
+int fmh_harmonic_shortcut_fails(float F0, int nb, double binHz, int nHarm)
+{
+  using namespace osm::hm;
+  const int last0 = freq_to_bin(binHz, nb, 0.5f * F0, 1);
+  for (int i = 0; i < nHarm; i++) {
+    const int prev = i == 0 ? last0 : freq_to_bin(binHz, nb, (float)i * F0, 0);
+    if (freq_to_bin(binHz, nb, (float)(i + 1) * F0, prev) != freq_to_bin(binHz, nb, (float)(i + 1) * F0, 0)) return i;
+  }
+  return -1;
+}
+
+// the product's window table (tables.cpp build_window), as the plan's windower level applies it
+void fmh_window(int winFunc, int N, double sigma, double gain, float *w)
+{
+  const double al[4] = {0.16, 0.0, 0.0, 0.0};
+  std::vector<float> v;
+  osm::build_window(winFunc, N, sigma, gain, v, al, 0, 0.0);
+  for (int n = 0; n < N; n++) w[n] = v[n];
+}
+
+// PCM -> cFormantLpc rows of T frames through formant_kernel's statements.  x = the mono float samples of the wave level (the
+// caller converts and mixes down as td_pcm does), frames of N samples every S, windowed as FrameReader::at (x w + offset);
+// then fmh_resample's transform / inverse sum, the autocorrelation, Durbin, the roots and emit().  out[T][nOut] with
+// nOut = [nValid] | formants[nF] | bandwidths[nF] (nF = the clamped nFormants); res[T][I] and lpc[T][p] when not null.
+// Returns nOut, or -1 where the graph pass refuses the geometry.
+int fmh_formant_rows(const float *x, int N, int S, int T, const float *win, float winOffset, double sampleRate, int nfft,
+                     double frameSizeSec, int zeroPadSymmetric, double targetFs, int p, int nFormants, double minF, double maxF,
+                     int saveNValid, int saveFormants, int saveBandwidths, float *out, float *resOut, float *lpcOut)
+{
+  osm::FormantOp op;
+  if (!formant_op(sampleRate, N, nfft, frameSizeSec, zeroPadSymmetric, targetFs, p, nFormants, minF, maxF, saveNValid, saveFormants,
+                  saveBandwidths, op)) return -1;
+  const int I = op.nRes, nF = op.nFormants;
+  std::vector<float> xw((size_t)N), res((size_t)I), a(p), fq(nF), bw(nF);
+  for (int t = 0; t < T; t++) {
+    for (int m = 0; m < N; m++) xw[m] = x[(size_t)t * S + m] * win[m] + winOffset;
+    resample_frames(op, N, xw.data(), 1, res.data());
+    fmh_lpc(res.data(), I, p, a.data());
+    const int nv = fmh_formants(a.data(), p, op.T, nF, minF, maxF, fq.data(), bw.data());
+    float *dst = out + (size_t)t * op.nOut;
+    int o = 0;
+    if (op.saveNValid) dst[o++] = (float)nv;
+    if (op.saveFormants) for (int i = 0; i < nF; i++) dst[o++] = fq[i];
+    if (op.saveBandwidths) for (int i = 0; i < nF; i++) dst[o++] = bw[i];
+    if (resOut) for (int i = 0; i < I; i++) resOut[(size_t)t * I + i] = res[i];
+    if (lpcOut) for (int i = 0; i < p; i++) lpcOut[(size_t)t * p + i] = a[i];
+  }
+  return op.nOut;
 }
 
 }
