@@ -22,7 +22,7 @@ OK, ERR_INVALID, ERR_UNSUPPORTED, ERR_CUDA, ERR_NOMEM = range(5)
  C_MELSPEC, C_MFCC, C_PLP, C_SPECTRAL, C_ENERGY, C_MZCR, C_ACF, C_PITCHACF,
  C_DELTAREGRESSION, C_CONTOURSMOOTHER, C_VECTORCONCAT, C_VECTOROPERATION, C_FULLINPUTMEAN, C_INTENSITY,
  C_SPECSCALE, C_PITCHSHS, C_PITCHSMOOTHERVITERBI, C_VALBASEDSELECTOR, C_PITCHJITTER,
- C_SPECRESAMPLE, C_LPC, C_FORMANTLPC, C_DATASELECTOR, C_HARMONICS, C_LSP, C_TONESPEC, C_CHROMA) = range(33)
+ C_SPECRESAMPLE, C_LPC, C_FORMANTLPC, C_DATASELECTOR, C_HARMONICS, C_LSP, C_TONESPEC, C_CHROMA, C_TONEFILT) = range(34)
 
 # cTonespec.filterType (osm_b200_tone_filter)
 TONE_GAU, TONE_TRI, TONE_TRP, TONE_REC = range(4)
@@ -40,7 +40,7 @@ TYPE_BY_NAME = {
     "cValbasedSelector": C_VALBASEDSELECTOR, "cPitchJitter": C_PITCHJITTER,
     "cSpecResample": C_SPECRESAMPLE, "cLpc": C_LPC, "cFormantLpc": C_FORMANTLPC,
     "cDataSelector": C_DATASELECTOR, "cHarmonics": C_HARMONICS, "cLsp": C_LSP,
-    "cTonespec": C_TONESPEC, "cChroma": C_CHROMA,
+    "cTonespec": C_TONESPEC, "cChroma": C_CHROMA, "cTonefilt": C_TONEFILT,
 }
 
 WIN_BY_NAME = {"rec": 0, "han": 1, "ham": 2, "gau": 3, "sin": 4, "tri": 5, "bar": 6}
@@ -233,6 +233,10 @@ class Chroma(C.Structure):
     _fields_ = [("octaveSize", i32), ("silThresh", f64)]
 
 
+class Tonefilt(C.Structure):
+    _fields_ = [("nNotes", i32), ("firstNote", f64), ("decayF0", f64), ("decayFN", f64), ("outputPeriod", f64)]
+
+
 class _U(C.Union):
     _fields_ = [("wavesource", WaveSource), ("framer", Framer),
                 ("vectorpreemphasis", VectorPreemphasis), ("windower", Windower),
@@ -245,7 +249,7 @@ class _U(C.Union):
                 ("valbasedselector", ValbasedSelector), ("pitchjitter", PitchJitter),
                 ("specresample", SpecResample), ("lpc", Lpc), ("formantlpc", FormantLpc),
                 ("dataselector", DataSelector), ("harmonics", Harmonics), ("lsp", Lsp),
-                ("tonespec", Tonespec), ("chroma", Chroma)]
+                ("tonespec", Tonespec), ("chroma", Chroma), ("tonefilt", Tonefilt)]
 
 
 class Component(C.Structure):
@@ -274,7 +278,7 @@ EXPORTS = [
     "osm_b200_abi_version", "osm_b200_sizeof_component", "osm_b200_last_error",
     "osm_b200_device_count", "osm_b200_component_defaults", "osm_b200_plan_create",
     "osm_b200_plan_destroy", "osm_b200_plan_num_elements", "osm_b200_plan_element_name",
-    "osm_b200_plan_frame_period", "osm_b200_plan_frame_size_samples",
+    "osm_b200_plan_frame_period", "osm_b200_plan_row_time", "osm_b200_plan_frame_size_samples",
     "osm_b200_plan_frame_step_samples", "osm_b200_plan_fft_size", "osm_b200_plan_num_frames", "osm_b200_plan_num_time_frames",
     "osm_b200_plan_frame_offsets", "osm_b200_plan_run_device", "osm_b200_plan_run_host", "osm_b200_plan_run_host_resident",
     "osm_b200_window_table", "osm_b200_tone_tables", "osm_b200_plan_num_frames_first_eoi", "osm_b200_plan_num_frames_first_eoi_v", "osm_b200_plan_copy_seq_lag",
@@ -325,6 +329,8 @@ def lib():
     L.osm_b200_plan_element_name.restype = C.c_char_p
     L.osm_b200_plan_frame_period.argtypes = [vp]
     L.osm_b200_plan_frame_period.restype = f64
+    L.osm_b200_plan_row_time.argtypes = [vp, C.c_int64]
+    L.osm_b200_plan_row_time.restype = f64
     for fn in ("frame_size_samples", "frame_step_samples", "fft_size", "last_launch_count"):
         getattr(L, "osm_b200_plan_" + fn).argtypes = [vp]
         getattr(L, "osm_b200_plan_" + fn).restype = i32
@@ -366,8 +372,8 @@ def lib():
         raise RuntimeError("ABI mismatch: sizeof(osm_b200_component) = %d, ctypes mirror = %d"
                            % (L.osm_b200_sizeof_component(), C.sizeof(Component)))
     L.osm_b200_tone_tables.argtypes = [C.POINTER(Tonespec), i32, f64, vp, vp, vp, vp, vp]
-    if L.osm_b200_component_defaults(C_CHROMA, C.byref(Component())) != 0:     # the last component type of this mirror
-        raise RuntimeError("ABI mismatch: the library does not know component type %d (cChroma)" % C_CHROMA)
+    if L.osm_b200_component_defaults(C_TONEFILT, C.byref(Component())) != 0:     # the last component type of this mirror
+        raise RuntimeError("ABI mismatch: the library does not know component type %d (cTonefilt)" % C_TONEFILT)
     _lib = L
     return L
 

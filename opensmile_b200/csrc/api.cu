@@ -16,6 +16,7 @@
 #include "cuda_owned.hpp"
 #include "kernels.cuh"
 #include "plan.hpp"
+#include "tonefilt_math.cuh"
 
 using namespace osm;
 
@@ -144,6 +145,12 @@ struct OpRt {
   DevBuf<unsigned char> dPitchTab;      // spline / interpolation / harmonic tables of the chain
   DevBuf<float> dShs;                   // [static rows][nShsCols] cPitchShs level
   DevBuf<int> dLag;                     // [nUtt] frames of the Viterbi level before the end-of-input flush
+  // cTonefilt (SOP_TONEFILT): block tables, segments of the prepared batch and their states
+  TonefiltParams tf;
+  DevBuf<double> dTfTab;                // W | a | freq
+  PinBuf<ChunkRef> hSegs; DevBuf<ChunkRef> dSegs;
+  std::vector<int32_t> uttSeg0; DevBuf<int32_t> dUttSeg0;
+  DevBuf<double2> dAgg, dCin;
   int descOp = -1;                      // index into PlanDesc::ops
 };
 
@@ -308,6 +315,10 @@ osm_b200_status osm_b200_component_defaults(int32_t type, osm_b200_component *c)
       c->u.tonespec.nOctaves = 6; c->u.tonespec.firstNote = 55.0; c->u.tonespec.filterType = OSM_B200_TONE_GAU; c->u.tonespec.dbA = 1;
       break;
     case OSM_B200_C_CHROMA: c->u.chroma.octaveSize = 12; c->u.chroma.silThresh = 0.001; c->copyInputName = 0; break;   // lld/chroma.cpp:46-49
+    case OSM_B200_C_TONEFILT:              // lld/tonefilt.cpp:35-41
+      c->u.tonefilt.nNotes = 48; c->u.tonefilt.firstNote = 55.0; c->u.tonefilt.decayF0 = 0.9995; c->u.tonefilt.decayFN = 0.998;
+      c->u.tonefilt.outputPeriod = 0.1;
+      break;
     case OSM_B200_C_HARMONICS: {           // lld/harmonics.cpp:28-56
       auto &q = c->u.harmonics;
       snprintf(q.f0ElementName, sizeof q.f0ElementName, "%s", "F0final");
@@ -825,6 +836,27 @@ static osm_b200_status build_time_op(const PlanDesc &d, const StaticOp &op, cons
   return OSM_B200_OK;
 }
 
+// cTonefilt [-> cChroma]: the block tables of tonefilt_math.cuh on the device
+static osm_b200_status build_tonefilt_rt(const PlanDesc &d, const StaticOp &op, const FrontEnd &fe, OpRt &rt)
+{
+  const TonefiltOp &to = op.tonefilt;
+  std::vector<double> W, a;
+  tf::block_tables(to.freq, to.decay, to.P, to.T, W, a);
+  std::vector<double> tab(W);
+  tab.insert(tab.end(), a.begin(), a.end());
+  tab.insert(tab.end(), to.freq.begin(), to.freq.end());
+  CU(rt.dTfTab.upload(tab.data(), tab.size()));
+  TonefiltParams &p = rt.tf;
+  memset(&p, 0, sizeof p);
+  p.tp.nChan = kernel_nchan(fe); p.tp.pcmF32 = fe.format != OSM_B200_PCM_S16; p.tp.statStride = d.nStatic; p.tp.outCol = op.outCol;
+  p.W = rt.dTfTab.p; p.nc = tf::padded_cols(to.nNotes); p.kp = tf::padded_rows(to.P);
+  p.a = rt.dTfTab.p + W.size(); p.freq = p.a + to.nNotes;
+  p.P = to.P; p.nNotes = to.nNotes; p.T = to.T;
+  p.chromaK = to.octaveSize; p.silThresh = to.silThresh;
+  tonefilt_smem_bytes(to.nNotes, to.octaveSize > 0, &p.smemSums);
+  return OSM_B200_OK;
+}
+
 // no exception crosses the C boundary (host allocation failures while the plan is built)
 osm_b200_status osm_b200_plan_create(const osm_b200_component *comps, int32_t n_comps,
                                      const char *output_level, int32_t device, osm_b200_plan **out)
@@ -889,7 +921,7 @@ try {
     OpRt rt;
     rt.kind = op.kind; rt.stream = op.stream; rt.descOp = (int)oi;
     StreamRt &srt = pl->st[op.stream];
-    if (op.kind != SOP_VECOP) srt.needTiles = true;      // the op reads its stream tile by tile
+    if (op.kind != SOP_VECOP && op.kind != SOP_TONEFILT) srt.needTiles = true;      // the op reads its stream tile by tile
     if (op.kind == SOP_MAG) {
       rt.vN = d.streams[op.stream].fe.nBins; rt.vOutCol = op.outCol;
       rt.magMode = op.magMode; rt.magN = (float)d.streams[op.stream].fe.nfft; rt.magDbNorm = op.magDbNorm; rt.magMinDb = op.magMinDb;
@@ -905,6 +937,7 @@ try {
         case SOP_PITCH: st = build_shs_chain(d, op, fe, srt, prop, rt); break;
         case SOP_JITTER: st = build_jitter(d, op, fe, rt); break;
         case SOP_PITCHACF: st = build_acf_pitch(d, op, fe, srt, rt); break;
+        case SOP_TONEFILT: st = build_tonefilt_rt(d, op, fe, rt); break;
         default: st = build_time_op(d, op, fe, srt, rt); break;
       }
       if (st != OSM_B200_OK) return st;
@@ -944,6 +977,12 @@ const char *osm_b200_plan_element_name(const osm_b200_plan *pl, int32_t idx)
 }
 
 double osm_b200_plan_frame_period(const osm_b200_plan *pl) { return pl ? pl->d.fe0().frameStepSec : 0.0; }
+double osm_b200_plan_row_time(const osm_b200_plan *pl, int64_t r)
+{
+  if (!pl) return 0.0;
+  const FrontEnd &fe = pl->d.fe0();
+  return fe.rowSampleStep > 0 ? (double)(r * fe.rowSampleStep) * (1.0 / fe.sampleRate) : (double)r * fe.frameStepSec;
+}
 int32_t osm_b200_plan_frame_size_samples(const osm_b200_plan *pl) { return pl ? pl->d.fe0().frameSize : 0; }
 int32_t osm_b200_plan_frame_step_samples(const osm_b200_plan *pl) { return pl ? pl->d.fe0().frameStep : 0; }
 int32_t osm_b200_plan_fft_size(const osm_b200_plan *pl) { return pl ? pl->d.fe0().nfft : 0; }
@@ -1056,6 +1095,31 @@ static osm_b200_status prepare_batch(osm_b200_plan *pl, const int64_t *uttOff, i
         CU(rt.dTiles.reserve(tiles.size() + 1));
         if (!tiles.empty()) CU(cudaMemcpyAsync(rt.dTiles.p, rt.hTiles.p, tiles.size() * sizeof(OpTile), cudaMemcpyHostToDevice, st));
       }
+    }
+    // cTonefilt segments: an utterance of up to kTfWhole rows is one segment, a longer one is cut every kTfSeg rows (the cut depends
+    // on the utterance alone: its rows do not depend on the batch)
+    for (OpRt &o : pl->ops) {
+      if (o.kind != SOP_TONEFILT) continue;
+      constexpr int64_t kTfWhole = 1024, kTfSeg = 128;
+      std::vector<ChunkRef> segs;
+      o.uttSeg0.assign(nm, 0);
+      for (int u = 0; u < nUtt; u++) {
+        o.uttSeg0[u] = (int32_t)segs.size();
+        const int64_t Tu = desc_num_static_frames(d, o.stream, uttOff[u + 1] - uttOff[u]);
+        const int64_t step = Tu <= kTfWhole ? kTfWhole : kTfSeg;
+        for (int64_t a = 0; a < Tu; a += step) segs.push_back(ChunkRef{u, (int32_t)a, (int32_t)std::min<int64_t>(a + step, Tu), 0, 0});
+      }
+      o.uttSeg0[nUtt] = (int32_t)segs.size();
+      const size_t ns = segs.size();
+      CU(o.hSegs.reserve(ns + 1));
+      if (ns) memcpy(o.hSegs.p, segs.data(), ns * sizeof(ChunkRef));
+      CU(o.dSegs.reserve(ns + 1));
+      if (ns) CU(cudaMemcpyAsync(o.dSegs.p, o.hSegs.p, ns * sizeof(ChunkRef), cudaMemcpyHostToDevice, st));
+      CU(o.dUttSeg0.reserve(nm));
+      CU(cudaMemcpyAsync(o.dUttSeg0.p, o.uttSeg0.data(), nm * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+      CU(o.dAgg.reserve(ns * o.tf.nNotes + 1));
+      CU(o.dCin.reserve(ns * o.tf.nNotes + 1));
+      pl->totalWork += ns;
     }
     pl->totalRows = hR[nUtt];
     pl->totalStat = hS[nUtt];
@@ -1175,6 +1239,21 @@ static osm_b200_status launch_range(osm_b200_plan *pl, const void *d_pcm, float 
       forked = true;
     }
     if (o.kind == SOP_HARMONICS) continue;              // reads the pitch and formant columns: launched after the join below
+    if (o.kind == SOP_TONEFILT) {
+      const int s0 = o.uttSeg0[u0], s1 = o.uttSeg0[u1];
+      if (s1 <= s0) continue;
+      bool carry = false;
+      for (int u = u0; u < u1 && !carry; u++) carry = o.uttSeg0[u + 1] - o.uttSeg0[u] > 1;
+      TonefiltParams tp = o.tf;
+      tp.tp.pcm = reinterpret_cast<const int16_t *>(d_pcm);
+      tp.tp.uttOff = dU; tp.tp.statOff = dS; tp.tp.stat = pl->dStat.p;
+      tp.segs = o.dSegs.p + s0; tp.nSegs = s1 - s0;
+      tp.agg = o.dAgg.p + (size_t)s0 * tp.nNotes; tp.cin = o.dCin.p + (size_t)s0 * tp.nNotes;
+      CU(launch_tonefilt(tp, o.dUttSeg0.p, u0, u1, carry, st));
+      pl->lastLaunches += carry ? 3 : 1;
+      PROF("tonefilt_kernel");
+      continue;
+    }
     cudaStream_t ks = (forked && (o.kind == SOP_PITCH || o.kind == SOP_JITTER)) ? pl->auxStream : st;
     if (o.kind == SOP_VECOP) {
       const long long *hS = pl->hMeta.p + 2 * nm;

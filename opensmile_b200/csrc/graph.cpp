@@ -34,7 +34,7 @@ const char *type_name(int t)
     "cMZcr", "cAcf", "cPitchACF", "cDeltaRegression", "cContourSmoother", "cVectorConcat",
     "cVectorOperation", "cFullinputMean", "cIntensity", "cSpecScale", "cPitchShs", "cPitchSmootherViterbi",
     "cValbasedSelector", "cPitchJitter", "cSpecResample", "cLpc", "cFormantLpc", "cDataSelector", "cHarmonics", "cLsp",
-    "cTonespec", "cChroma"};
+    "cTonespec", "cChroma", "cTonefilt"};
   return (t >= 0 && t < OSM_B200_C_COUNT_) ? names[t] : "?";
 }
 
@@ -50,6 +50,7 @@ const char *default_name_append(int t)
     case OSM_B200_C_ENERGY: return "energy";
     case OSM_B200_C_TONESPEC: return "note";       // lld/tonespec.cpp:47
     case OSM_B200_C_CHROMA: return "chroma";       // lld/chroma.cpp:46
+    case OSM_B200_C_TONEFILT: return "tonefilt";   // lld/tonefilt.cpp:35
     default: return "";
   }
 }
@@ -70,7 +71,9 @@ std::string name_append_auto(const osm_b200_component &c, const std::string &bas
 }  // namespace
 
 // core/winToVecProcessor.cpp:868-877 (noPostEOIprocessing=1, frameCenterSpecial=left):
-// only complete frames => T = floor((L - size)/step) + 1
+// only complete frames => T = floor((L - size)/step) + 1.
+// A cTonefilt stream (GraphCompiler::get_tonefilt_stream) reads blocks of P samples with hop P and gets one more, padded block
+// for a remainder at end of input: ceil(L / P) rows, which is this rule for a "frame" of 1 sample and a step of P.
 int64_t desc_num_static_frames(const PlanDesc &d, int stream, int64_t L)
 {
   const FrontEnd &fe = d.streams[stream].fe;
@@ -436,6 +439,7 @@ struct GraphCompiler {
       case OSM_B200_C_VALBASEDSELECTOR: case OSM_B200_C_PITCHSMOOTHERVITERBI: case OSM_B200_C_PITCHSHS: s = build_pitch_chain_op(c, op); break;
       case OSM_B200_C_PITCHJITTER: s = build_jitter_op(c, op); break;
       case OSM_B200_C_TONESPEC: case OSM_B200_C_CHROMA: s = build_tone_op(c, op); break;
+      case OSM_B200_C_TONEFILT: s = build_tonefilt_op(c, op); break;
       default: {
         char buf[512];
         snprintf(buf, sizeof buf, "component '%s' (%s) is not a supported static LLD producer", c->name, type_name(c->type));
@@ -955,7 +959,8 @@ struct GraphCompiler {
     const osm_b200_component *ts = c;
     if (c->type == OSM_B200_C_CHROMA) {
       ts = single_input(c);
-      if (!ts || ts->type != OSM_B200_C_TONESPEC) { err = "cChroma must read a cTonespec level"; return OSM_B200_ERR_UNSUPPORTED; }
+      if (ts && ts->type == OSM_B200_C_TONEFILT) return build_tonefilt_op(c, op);
+      if (!ts || ts->type != OSM_B200_C_TONESPEC) { err = "cChroma must read a cTonespec level (or a cTonefilt level)"; return OSM_B200_ERR_UNSUPPORTED; }
     }
     ChainInfo ci;
     if (!resolve_mag_chain(single_input(ts), ci)) { err = "cTonespec: " + err; return OSM_B200_ERR_UNSUPPORTED; }
@@ -980,6 +985,64 @@ struct GraphCompiler {
     to.silThresh = (float)q.silThresh;                                                     // :71
     to.nOut = q.octaveSize;
     add_field(op, name_append_auto(*c, toneName, nullptr), q.octaveSize);                 // :78-81
+    return OSM_B200_OK;
+  }
+
+  // cTonefilt on the wave level, or cChroma on such a cTonefilt level (config/chroma/chroma_filt.conf): a stream of its own whose
+  // rows are blocks of P samples (tonefilt.cu)
+  osm_b200_status build_tonefilt_op(const osm_b200_component *c, StaticOp &op)
+  {
+    const osm_b200_component *tfc = c->type == OSM_B200_C_CHROMA ? single_input(c) : c;
+    const osm_b200_component *wv = single_input(tfc);
+    if (!wv || wv->type != OSM_B200_C_WAVESOURCE) {
+      err = "cTonefilt must read the cWaveSource level (on a frame level it would filter every element as a signal of its own)";
+      return OSM_B200_ERR_UNSUPPORTED;
+    }
+    const auto &wp = wv->u.wavesource;
+    if (wp.nChannels > 1 && !wp.monoMixdown) { err = "cTonefilt: a multi-element wave level (monoMixdown = 0) is not supported"; return OSM_B200_ERR_UNSUPPORTED; }
+    if (wp.sampleRate <= 0) { err = "cWaveSource: bad sampleRate/nChannels"; return OSM_B200_ERR_INVALID; }
+    op.kind = SOP_TONEFILT;
+    TonefiltOp &to = op.tonefilt;
+    if (!build_tonefilt(tfc->u.tonefilt, wp.sampleRate, to, err)) return OSM_B200_ERR_UNSUPPORTED;
+    osm_b200_status s2 = get_tonefilt_stream(wv, tfc, to, op.stream);
+    if (s2 != OSM_B200_OK) return s2;
+    // <input field>_<nameAppend> with nNotes elements; copyInputName plays no part (lld/tonefilt.cpp:137-172)
+    const std::string na = tfc->nameAppend[0] ? tfc->nameAppend : default_name_append(OSM_B200_C_TONEFILT);
+    const std::string tfName = wave_name(ChainInfo{wv}) + "_" + na;
+    if (c->type == OSM_B200_C_TONEFILT) {
+      add_field(op, tfName, to.nNotes);
+      return OSM_B200_OK;
+    }
+    if (to.nNotes == 1) {                                              // core/vectorProcessor.cpp:196-243
+      err = "cChroma on a one-note cTonefilt level: the reference's cChroma (processArrayFields = 1) finds no array field there"; return OSM_B200_ERR_UNSUPPORTED;
+    }
+    const auto &q = c->u.chroma;
+    if (q.octaveSize < 1 || to.nNotes % q.octaveSize != 0) {           // lld/chroma.cpp:94-115
+      err = "cChroma.octaveSize must divide the number of cTonefilt notes (nNotes)"; return OSM_B200_ERR_UNSUPPORTED;
+    }
+    to.octaveSize = q.octaveSize;
+    to.silThresh = (float)q.silThresh;                                 // :71
+    add_field(op, name_append_auto(*c, tfName, nullptr), q.octaveSize); // :78-81
+    return OSM_B200_OK;
+  }
+
+  // the stream of a cTonefilt level: the wave format of the source, rows = blocks of P samples with hop P, period outputPeriod
+  // (lld/tonefilt.cpp:101-134).  The row rule of desc_num_static_frames gives ceil(L / P) with frameSize 1 and frameStep P.
+  osm_b200_status get_tonefilt_stream(const osm_b200_component *wv, const osm_b200_component *tfc, const TonefiltOp &to, int &idx)
+  {
+    for (size_t s = 0; s < d.streams.size(); s++)
+      if (d.streams[s].keyFramer == tfc) { idx = (int)s; return OSM_B200_OK; }
+    const auto &wp = wv->u.wavesource;
+    if (wp.format < OSM_B200_PCM_S16 || wp.format > OSM_B200_PCM_S32) { err = "cWaveSource: unknown sample format"; return OSM_B200_ERR_INVALID; }
+    Stream st;
+    FrontEnd &fe = st.fe;
+    fe.sampleRate = wp.sampleRate; fe.nChan = wp.nChannels; fe.format = wp.format; fe.mixdown = true;
+    fe.frameSize = 1; fe.frameStep = to.P;
+    fe.frameSizeSec = to.period; fe.frameStepSec = to.period;
+    fe.rowSampleStep = to.P;
+    st.keyFramer = tfc;
+    d.streams.push_back(st);
+    idx = (int)d.streams.size() - 1;
     return OSM_B200_OK;
   }
 

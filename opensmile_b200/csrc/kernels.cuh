@@ -278,6 +278,25 @@ cudaError_t launch_harmonics(const HarmonicsParams &p, cudaStream_t st);
 size_t harmonics_smem_bytes(const HarmonicsParams &p);
 
 // ------------------------------------------------------------------------------------------
+// cTonefilt [-> cChroma] on the wave level (tonefilt.cu, tonefilt_math.cuh): one CTA per segment of rows (blocks of P samples)
+// of one utterance; the in-block sums are one FP64 tensor-core product with the table W, the blocks are chained per note
+// ------------------------------------------------------------------------------------------
+struct TonefiltParams {
+  TimeOpParams tp;               // pcm, nChan, pcmF32, uttOff, statOff, stat, statStride, outCol (frame fields unused)
+  const ChunkRef *segs; int nSegs;   // segments: rows [a, b) of utterance utt
+  const double *W; int nc, kp;   // [kp][nc]: w_j of every note, re / im interleaved, zero-padded (tonefilt_math.cuh block_tables)
+  const double *a, *freq;        // [nNotes] d^P, note frequency
+  int P, nNotes; double T;       // samples per block, notes, period of the wave level
+  double2 *agg, *cin;            // [nSegs][nNotes] end state of a segment from a zero state / state entering it
+  int chromaK; float silThresh;  // chromaK > 0: cChroma behind the filter bank (octaveSize), 0: the tone values are the output
+  size_t smemSums;               // byte offset of the chroma staging area in shared memory (tonefilt_smem_bytes)
+};
+// uttSeg0[u] = first segment of utterance u (absolute); p.segs / agg / cin start at segment uttSeg0[u0].  carry = some utterance of
+// [u0, u1) has more than one segment: the aggregate pass and the carry kernel run first.
+cudaError_t launch_tonefilt(const TonefiltParams &p, const int32_t *uttSeg0, int u0, int u1, bool carry, cudaStream_t st);
+size_t tonefilt_smem_bytes(int nNotes, int chroma, size_t *sumsOffset);
+
+// ------------------------------------------------------------------------------------------
 // SHS pitch chain (pitch.cu): cSpecScale + cPitchShs per frame (one warp per frame), cPitchSmootherViterbi
 // [+ cValbasedSelector] per utterance (one thread), cPitchJitter per utterance (one warp), and the temporal
 // stages of the levels behind them (one thread per utterance, seq_post_kernel).

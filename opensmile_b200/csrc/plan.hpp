@@ -46,6 +46,17 @@ struct ToneOp {
   int nOut = 0;
 };
 
+// cTonefilt (lld/tonefilt.cpp:65-189) after the reference's clamps, and an optional cChroma behind it
+struct TonefiltOp {
+  int nNotes = 0;
+  int P = 1;                           // samples per output row (configureWriter, :101-134)
+  double T = 0;                        // period of the wave level
+  double period = 0;                   // outputPeriod: period and frame size of the level
+  std::vector<double> freq, decay;     // [nNotes] (:180-189)
+  int octaveSize = 0;                  // > 0: cChroma behind the filter bank
+  float silThresh = 0.f;
+};
+
 struct FrontEnd {
   double sampleRate = 0;
   int nChan = 1;
@@ -61,9 +72,12 @@ struct FrontEnd {
   std::vector<float> window;       // (float)win[n], size frameSize (windower.cpp:226)
   float winOffset = 0.f;
   bool zeroPadSymmetric = false;   // phase only; magnitude consumers are unaffected
+  // cTonefilt rows: the time of row r is that of its first sample, (double)(r * rowSampleStep) / fs (lld/tonefilt.cpp:252,
+  // core/dataMemoryLevel.cpp:617-626, 1240); 0: a framer level, r * frameStepSec
+  int rowSampleStep = 0;
 };
 
-enum StaticOpKind { SOP_MFCC = 0, SOP_PLP, SOP_MELSPEC, SOP_SPECTRAL, SOP_ENERGY, SOP_MZCR, SOP_PITCHACF, SOP_VECOP, SOP_MAG, SOP_INTENSITY, SOP_PITCH, SOP_JITTER, SOP_FORMANT, SOP_HARMONICS, SOP_LPC, SOP_TONE };
+enum StaticOpKind { SOP_MFCC = 0, SOP_PLP, SOP_MELSPEC, SOP_SPECTRAL, SOP_ENERGY, SOP_MZCR, SOP_PITCHACF, SOP_VECOP, SOP_MAG, SOP_INTENSITY, SOP_PITCH, SOP_JITTER, SOP_FORMANT, SOP_HARMONICS, SOP_LPC, SOP_TONE, SOP_TONEFILT };
 
 struct MfccOp {
   int melIdx = 0;
@@ -238,6 +252,7 @@ struct StaticOp {
   HarmonicsOp harmonics;
   LpcOp lpc;
   ToneOp tone;
+  TonefiltOp tonefilt;
 };
 
 // temporal stage applied to a static column range (cWindowProcessor family)
@@ -308,6 +323,8 @@ void build_energy(const osm_b200_energy &cfg, EnergyOp &op);
 bool build_tone_tables(const osm_b200_tonespec &cfg, int nBins, double fftFrameSizeSec, ToneTables &t, std::string &err);
 bool build_tone(const osm_b200_tonespec &cfg, int nBins, double fftFrameSizeSec, ToneOp &op, std::string &err);
 void build_mzcr(const osm_b200_mzcr &cfg, MzcrOp &op);
+// cTonefilt on a wave level of sampling rate fs: the reference's clamps, block length and tables; false (err set) where unsupported
+bool build_tonefilt(const osm_b200_tonefilt &cfg, double fs, TonefiltOp &op, std::string &err);
 // vc == nullptr: the op stops at the cPitchShs level (PitchChainOp::shsOnly)
 bool build_pitch_chain(const osm_b200_specscale &sc, const osm_b200_pitchshs &ps, const osm_b200_pitchsmootherviterbi *vc,
                        int nMag, double fftFrameSizeSec, PitchChainOp &op, std::string &err);

@@ -474,6 +474,34 @@ void build_mzcr(const osm_b200_mzcr &cfg, MzcrOp &op)
   op.nOut = (int)op.zcr + (int)op.mcr + (int)op.amax + 2 * (int)op.maxmin + (int)op.dc;
 }
 
+// cTonefilt::myFetchConfig (lld/tonefilt.cpp:65-98), configureWriter (:101-134) and the tables of setupNewNames (:180-189)
+bool build_tonefilt(const osm_b200_tonefilt &cfg, double fs, TonefiltOp &op, std::string &err)
+{
+  double period = cfg.outputPeriod;
+  if (period <= 0.0) period = 0.1;
+  double dN = cfg.decayFN;
+  if (dN < 0.0) dN = 0.0;
+  if (dN > 1.0) dN = 1.0;
+  double d0 = cfg.decayF0;
+  if (d0 < dN) d0 = dN;
+  if (d0 < 0.0) d0 = 0.0;
+  if (d0 > 1.0) d0 = 1.0;
+  double first = cfg.firstNote;
+  if (first <= 0.0) first = 1.0;
+  int n = cfg.nNotes;
+  if (n < 1) n = 1;
+  if (n > 128) { err = "cTonefilt.nNotes above 128 is not supported"; return false; }
+  const double T = 1.0 / fs;                     // the wave level's period (iocore/waveSource.cpp)
+  long P = (long)round(period / T);
+  if (period < T) { period = T; P = 1; }
+  if (P < 1 || P > (1L << 20)) { err = "cTonefilt.outputPeriod out of the supported range"; return false; }
+  op.nNotes = n; op.P = (int)P; op.T = T; op.period = period;
+  op.freq.resize(n); op.decay.resize(n);
+  for (int k = 0; k < n; k++) op.freq[k] = first * pow(2.0, (double)k / 12.0);
+  for (int k = 0; k < n; k++) op.decay[k] = dN + (d0 - dN) * (op.freq[k] - op.freq[0]) / (op.freq[n - 1]);   // the last frequency, not the span
+  return true;
+}
+
 // cSpecScale::dataProcessorCustomFinalise (dsp/specScale.cpp:236-313), cPitchShs::setupNewNames
 // (lld/pitchShs.cpp:160-215), cPitchBase / cPitchSmootherViterbi configuration.  The spline's abscissa
 // terms (smileUtilSpline.c:124-140) are folded into recurrence coefficients, see PitchChainOp.

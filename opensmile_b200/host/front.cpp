@@ -238,7 +238,8 @@ const TypeInfo kTypes[] = {
   {"cPitchSmootherViterbi", OSM_B200_C_PITCHSMOOTHERVITERBI}, {"cValbasedSelector", OSM_B200_C_VALBASEDSELECTOR},
   {"cPitchJitter", OSM_B200_C_PITCHJITTER}, {"cSpecResample", OSM_B200_C_SPECRESAMPLE}, {"cLpc", OSM_B200_C_LPC},
   {"cFormantLpc", OSM_B200_C_FORMANTLPC}, {"cDataSelector", OSM_B200_C_DATASELECTOR},
-  {"cHarmonics", OSM_B200_C_HARMONICS}, {"cLsp", OSM_B200_C_LSP}, {"cTonespec", OSM_B200_C_TONESPEC}, {"cChroma", OSM_B200_C_CHROMA}};
+  {"cHarmonics", OSM_B200_C_HARMONICS}, {"cLsp", OSM_B200_C_LSP}, {"cTonespec", OSM_B200_C_TONESPEC}, {"cChroma", OSM_B200_C_CHROMA},
+  {"cTonefilt", OSM_B200_C_TONEFILT}};
 
 // cTonespec.filterType spellings (lld/tonespec.cpp:107-111); any other value leaves the constructor's Gaussian (:83)
 int tone_filter(const std::string &f)
@@ -635,6 +636,12 @@ bool to_component(const Section &s, osm_b200_component &c, std::string &err)
       case OSM_B200_C_CHROMA:               // lld/chroma.cpp:46-49
         SETI("octaveSize", c.u.chroma.octaveSize) SETD("silThresh", c.u.chroma.silThresh)
         break;
+      case OSM_B200_C_TONEFILT: {           // lld/tonefilt.cpp:35-41 (outputBuffersize is commented out there: unknown)
+        auto &q = c.u.tonefilt;
+        SETI("nNotes", q.nNotes) SETD("firstNote", q.firstNote) SETD("decayF0", q.decayF0) SETD("decayFN", q.decayFN)
+        SETD("outputPeriod", q.outputPeriod)
+        break;
+      }
       default: break;
     }
     // same behaviour as the reference: an unknown field aborts configuration (configManager.cpp:2599)
@@ -1090,8 +1097,17 @@ bool device_htk(const float *dRows, int64_t n, int K, std::vector<uint32_t> &pac
          cudaMemcpy(packed.data(), dPack.p, (size_t)n * K * 4, cudaMemcpyDeviceToHost) == cudaSuccess;
 }
 
+// time stamp of row r: min(r, nTimeFrames - 1) rows into the level, whose rows are `period` apart unless the plan says otherwise
+// (osm_b200_plan_row_time: cTonefilt rows carry the time of their first sample)
+static double row_time(int64_t r, int64_t nTimeFrames, double period, const osm_b200_plan *timePlan)
+{
+  const int64_t t = (nTimeFrames > 0 && r > nTimeFrames - 1) ? nTimeFrames - 1 : r;
+  return timePlan ? osm_b200_plan_row_time(timePlan, t) : (double)t * period;
+}
+
 bool write_csv(const char *path, const float *rows, int64_t n, int K, const std::vector<std::string> &names, double period,
-               const CsvOpts &o, std::string &err, int64_t nTimeFrames = 0, const DevText *dt = nullptr)
+               const CsvOpts &o, std::string &err, int64_t nTimeFrames = 0, const DevText *dt = nullptr,
+               const osm_b200_plan *timePlan = nullptr)
 {
   FILE *f = fopen(path, "w");
   if (!f) { err = std::string("cannot write '") + path + "'"; return false; }
@@ -1111,7 +1127,7 @@ bool write_csv(const char *path, const float *rows, int64_t n, int K, const std:
     }
     if (o.number) { tb.fmt_ld((long)r); tb.ch(o.delim); }
     // rows appended by a window processor at the end of input carry a copy of the last frame's time stamp
-    if (o.timestamp) { tb.fmt_f6((double)((nTimeFrames > 0 && r > nTimeFrames - 1) ? nTimeFrames - 1 : r) * period); tb.ch(o.delim); }
+    if (o.timestamp) { tb.fmt_f6(row_time(r, nTimeFrames, period, timePlan)); tb.ch(o.delim); }
     if (dt && !dt->host[r]) { tb.str(dt->text + r * dt->slot, (size_t)dt->len[r]); continue; }
     for (int k = 0; k < K; k++) {
       const float v = rows[r * K + k];
@@ -1154,7 +1170,8 @@ std::string arff_escape(const std::string &str)               // iocore/arffSink
 }
 
 bool write_arff(const char *path, const float *rows, int64_t n, int K, const std::vector<std::string> &names, double period,
-                const ArffOpts &o, std::string &err, int64_t nTimeFrames = 0, const DevText *dt = nullptr)
+                const ArffOpts &o, std::string &err, int64_t nTimeFrames = 0, const DevText *dt = nullptr,
+                const osm_b200_plan *timePlan = nullptr)
 {
   bool header = true;
   if (o.append) {                                             // :244-256: append to an existing file without a header
@@ -1181,7 +1198,7 @@ bool write_arff(const char *path, const float *rows, int64_t n, int K, const std
     if (o.prname == 1) fprintf(f, "%s,", arff_escape(o.instName).c_str());
     else if (o.prname == 2) { char b[512]; snprintf(b, sizeof b, "%s_%ld", o.instName.c_str(), (long)r); fprintf(f, "%s,", arff_escape(b).c_str()); }
     if (o.number) fprintf(f, "%ld,", (long)r);
-    if (o.timestamp) fprintf(f, "%f,", (double)((nTimeFrames > 0 && r > nTimeFrames - 1) ? nTimeFrames - 1 : r) * period + o.frameTimeAdd);
+    if (o.timestamp) fprintf(f, "%f,", row_time(r, nTimeFrames, period, timePlan) + o.frameTimeAdd);
     if (dt && !dt->host[r]) tb.str(dt->text + r * dt->slot, (size_t)dt->len[r] - 1);   // the device's row text without its newline
     else {
       tb.fmt_e(rows[r * K]);
@@ -1766,6 +1783,11 @@ try {
     const PlanPtr plan(p);
     if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
     if (s->hasFunc) {
+      // the summary is taken at the first end-of-input tick; how many cTonefilt rows exist then (its last, padded block is
+      // written only after end of input) is not modelled
+      for (const osm_b200_component &c : cs)
+        if (c.type == OSM_B200_C_TONEFILT)
+          return hfail(OSM_B200_ERR_UNSUPPORTED, std::string("cFunctionals reading a level behind cTonefilt '") + c.name + "' is not supported");
       osm_b200_session::FuncRt rt;
       st = build_func_rt(s.get(), 16000, 1, p, -1, rt);
       if (st != OSM_B200_OK) return hfail(st, osm_b200_host_last_error());
@@ -1982,10 +2004,10 @@ static bool write_batch(osm_b200_session *s, const std::vector<int> &idx, const 
     if (htkPaths && htkPaths[i] && !write_htk(htkPaths[i], r, nr, K, period, s->parmKind, e, packed ? packed + (size_t)fo[k] * K : nullptr)) return false;
     DevText dk;
     if (dt) dk = DevText{dt->text + fo[k] * dt->slot, dt->slot, dt->len + fo[k], dt->host + fo[k]};
-    if (csvPaths && csvPaths[i] && !write_csv(csvPaths[i], r, nr, K, names, period, s->csv, e, nTime[k], dt ? &dk : nullptr)) return false;
+    if (csvPaths && csvPaths[i] && !write_csv(csvPaths[i], r, nr, K, names, period, s->csv, e, nTime[k], dt ? &dk : nullptr, s->cur)) return false;
     DevText da;
     if (dtArff) da = DevText{dtArff->text + fo[k] * dtArff->slot, dtArff->slot, dtArff->len + fo[k], dtArff->host + fo[k]};
-    if (arffPaths && arffPaths[i] && !write_arff(arffPaths[i], r, nr, K, names, period, s->arff, e, nTime[k], dtArff ? &da : nullptr)) return false;
+    if (arffPaths && arffPaths[i] && !write_arff(arffPaths[i], r, nr, K, names, period, s->arff, e, nTime[k], dtArff ? &da : nullptr, s->cur)) return false;
     return true;
   }, err, shared);
 }
