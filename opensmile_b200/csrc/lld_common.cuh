@@ -454,12 +454,15 @@ __device__ __forceinline__ void emit_interior(const float *__restrict__ ring, fl
 // Fused delta / delta-delta emission, general path (utterance edges, deltawin != 2): lane = row, warps
 // take the coefficients; clamping and the tick-order model of post_kernel decide what a read past
 // either end of a level returns.  Out of line: it runs on the first / last tiles of an utterance only.
-template <int F, int NW>
+// KC / WC != 0: the coefficients K and both windows W1 = W2 known at compile time (lld_fast.cu), the
+// arguments K, W1, W2 are then not read.
+template <int F, int NW, int KC = 0, int WC = 0>
 __device__ OSM_COLD void emit_edge(const float *__restrict__ ring, float *__restrict__ Dbuf, float *__restrict__ outS,
-                               int K, int W1, int W2, int T, int T1, int c01, int c02, int s0, int r0, int r1,
+                               int Kr, int W1r, int W2r, int T, int T1, int c01, int c02, int s0, int r0, int r1,
                                int d0, int d1, int dRows, float norm1, float rcp1, float norm2, float rcp2,
                                int warp, int lane)
 {
+  const int K = KC ? KC : Kr, W1 = WC ? WC : W1r, W2 = WC ? WC : W2r;
   const int K3 = 3 * K, nr = r1 - r0;
   for (int c = warp; c < K; c += NW) {
     const float *rc = ring + c * (2 * F);

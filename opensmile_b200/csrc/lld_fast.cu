@@ -15,6 +15,8 @@
 //            same (a_q, b_{15-q}) pairing so that every warp executes the same code.
 //   mel      visit list read as float4 (two bins per load); the band level lives behind the power spectrum, not in the sample tile
 //   DCT      table transposed, [band][16]: a warp evaluates two coefficients per band value read, in the reference's order
+//   emit     with 13 static columns (lld512_kernel<NZR, 13>) every thread's Δ / ΔΔ items are fixed at compile time
+//   store    the tile's rows leave 16 bytes at a time (staged at their global offset modulo 16 bytes)
 //
 // Reference rows as in kernels.cu (SURVEY.md 8a-1 ... a-8, a-13, a-15).
 #include "lld_common.cuh"
@@ -99,7 +101,76 @@ __device__ __forceinline__ void split_pair(float2 a, float2 b, float2 w, float &
   pm = __fmaf_rn(yr, yr, __fmul_rn(yi, yi));
 }
 
-template <int NZR>
+// eight samples of a landing zone whose fetch did not start 16-byte aligned (the PCM buffer is not): four 32-bit words
+// from 16-bit loads, out of line -- a 16-byte aligned buffer never takes it
+static __device__ OSM_COLD int4 load8_unaligned(const int16_t *s)
+{
+  const unsigned short *up = reinterpret_cast<const unsigned short *>(s);
+  int w[4];
+#pragma unroll
+  for (int jj = 0; jj < 4; jj++) w[jj] = (int)((unsigned)up[2 * jj] | ((unsigned)up[2 * jj + 1] << 16));
+  return make_int4(w[0], w[1], w[2], w[3]);
+}
+
+// one 8-byte shared-memory store (STS.64).  The sample tile's pairs are 8-byte aligned -- i is a multiple of 8, sPad is even
+// (lld_fast_applies), the tile starts 16-byte aligned -- but the compiler cannot prove it and splits a float2 store in two.
+__device__ __forceinline__ void sts_f2(float *dst, float a, float b)
+{
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(smem_u32(dst)), "f"(a), "f"(b) : "memory");
+}
+
+// Fused Δ / ΔΔ emission of one interior tile (emit_interior of lld_common.cuh) with K static columns known at compile
+// time: every thread's items are fixed -- the delta items tid and tid + NT, the static / delta-delta items of columns
+// warp and warp + NW at row lane -- so the column / row split and the row offsets are constants of the thread, and only
+// the ring slots move from tile to tile.  Same statements, same order, same results as emit_interior.
+template <int K>
+__device__ __forceinline__ void delta_item(const float *__restrict__ ring, float *__restrict__ Dbuf, float *__restrict__ outS,
+                                           int slot0, float norm1, float rcp1, int item)
+{
+  constexpr int F = kF, DR = F + 4, dRows = F + 24, K3 = 3 * K, RM = 2 * F - 1;
+  const int c = item / DR, tt = item - c * DR;
+  const float *rc = ring + c * (2 * F);
+  const int sl = slot0 + tt;
+  const float dA = __fsub_rn(rc[(sl + 1) & RM], rc[(sl - 1) & RM]);
+  const float dB = __fsub_rn(rc[(sl + 2) & RM], rc[(sl - 2) & RM]);
+  const float dv = div_exact(__fadd_rn(dA, __fmul_rn(2.0f, dB)), norm1, rcp1);
+  Dbuf[c * dRows + tt] = dv;
+  const int rr = tt - 2;
+  if (rr >= 0 && rr < F) outS[rr * K3 + K + c] = dv;
+}
+
+template <int K>
+__device__ __forceinline__ void delta2_item(const float *__restrict__ Dbuf, float *__restrict__ outS, float norm2, float rcp2,
+                                            int c, int lane)
+{
+  constexpr int dRows = kF + 24, K3 = 3 * K;
+  const float *dt = Dbuf + c * dRows + lane + 2;                 // row t = r0 + lane sits at tt = lane + 2
+  const float dA = __fsub_rn(dt[1], dt[-1]);
+  const float dB = __fsub_rn(dt[2], dt[-2]);
+  outS[lane * K3 + 2 * K + c] = div_exact(__fadd_rn(dA, __fmul_rn(2.0f, dB)), norm2, rcp2);
+}
+
+template <int K>
+__device__ __forceinline__ void emit_interior_k(const float *__restrict__ ring, float *__restrict__ Dbuf,
+                                                float *__restrict__ outS, int slot0, int rslot0,
+                                                float norm1, float rcp1, float norm2, float rcp2, int tid)
+{
+  constexpr int F = kF, NT = kNT, NW = kNW, DR = F + 4, K3 = 3 * K, RM = 2 * F - 1;
+  static_assert(K * DR > NT && K * DR <= 2 * NT && K > NW && K <= 2 * NW, "two delta items and two columns per thread");
+  const int warp = tid >> 5, lane = tid & 31;
+  delta_item<K>(ring, Dbuf, outS, slot0, norm1, rcp1, tid);
+  if (tid < K * DR - NT) delta_item<K>(ring, Dbuf, outS, slot0, norm1, rcp1, tid + NT);
+  const float *rs = ring + ((rslot0 + lane) & RM);               // statics -> outS
+  outS[lane * K3 + warp] = rs[warp * (2 * F)];
+  if (warp + NW < K) outS[lane * K3 + warp + NW] = rs[(warp + NW) * (2 * F)];
+  __syncthreads();
+  delta2_item<K>(Dbuf, outS, norm2, rcp2, warp, lane);          // delta-delta rows
+  if (warp + NW < K) delta2_item<K>(Dbuf, outS, norm2, rcp2, warp + NW, lane);
+  __syncthreads();
+}
+
+// KC: the static columns of the fused Δ / ΔΔ emission when known at compile time (13: MFCC 0..12), 0 = p.nStat
+template <int NZR, int KC>
 __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
 {
   constexpr int M = kM, F = kF, NT = kNT, NW = kNW;
@@ -107,6 +178,7 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
 
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ ChunkCtx sCx[2];
+  __shared__ int sTg[3];                // count, mis, lead of the tile in the landing zone (TileGeom), set with its fetch
   __shared__ int sRun[2];
   const SmemLayout L = make_layout(p, M, F);
   float2 *Z = reinterpret_cast<float2 *>(smem + L.zbuf);
@@ -164,6 +236,7 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
   if (tid == 0) {
     sCx[0] = load_chunk<F>(p, chunk);
     const TileGeom g0 = tile_geom<F>(p, sCx[0], 0);
+    sTg[0] = g0.count; sTg[1] = g0.mis; sTg[2] = g0.lead;
     mbar_expect_tx(mbar, g0.bytes);
     bulk_g2s(rawPcm, g0.src, g0.bytes, mbar);
   }
@@ -185,23 +258,18 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
     mbar_wait(mbar, phase);
     phase ^= 1;
     {
-      const TileGeom tg = tile_geom<F>(p, cx, j);
-      const int count = tg.count;
-      const int16_t *rp = reinterpret_cast<const int16_t *>(rawPcm + tg.mis) + tg.lead;
-      const bool aligned = (tg.mis == 0);
-      const bool hasLead = tg.lead > 0;
+      // the tile's geometry comes from the thread that issued its fetch (sTg), not from every thread's 64-bit arithmetic
+      const int count = sTg[0], mis = sTg[1], lead = sTg[2];
+      const int16_t *rp = reinterpret_cast<const int16_t *>(rawPcm + mis) + lead;
+      const bool aligned = (mis == 0);
+      const bool hasLead = lead > 0;
       const float ks = p.preDe ? p.preK : -p.preK;
 #pragma unroll 1
       for (int i = tid * 8; i < count; i += NT * 8) {
-        int wds[4];
-        if (aligned) {
-          const int4 w4 = *reinterpret_cast<const int4 *>(rp + i);
-          wds[0] = w4.x; wds[1] = w4.y; wds[2] = w4.z; wds[3] = w4.w;
-        } else {
-          const unsigned short *up = reinterpret_cast<const unsigned short *>(rp + i);
-#pragma unroll
-          for (int jj = 0; jj < 4; jj++) wds[jj] = (int)((unsigned)up[2 * jj] | ((unsigned)up[2 * jj + 1] << 16));
-        }
+        int4 w4;
+        if (aligned) w4 = *reinterpret_cast<const int4 *>(rp + i);
+        else w4 = load8_unaligned(rp + i);
+        const int wds[4] = {w4.x, w4.y, w4.z, w4.w};
         float x[8], y[8];
 #pragma unroll
         for (int jj = 0; jj < 4; jj++) {
@@ -222,19 +290,21 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
         float *dst = samp + i + q * p.sPad;
         if (i == q * hop && q < F) raw[q] = x[0];                  // first sample of frame q, not pre-emphasised
 #pragma unroll
-        for (int jj = 0; jj < 8; jj += 2) *reinterpret_cast<float2 *>(dst + jj) = make_float2(y[jj], y[jj + 1]);
+        for (int jj = 0; jj < 8; jj += 2) sts_f2(dst + jj, y[jj], y[jj + 1]);
       }
     }
     __syncthreads();
     if (tid == 0) {
       if (j + 1 < cx.nT) {
         const TileGeom gn = tile_geom<F>(p, cx, j + 1);
+        sTg[0] = gn.count; sTg[1] = gn.mis; sTg[2] = gn.lead;     // read after this tile's barriers
         mbar_expect_tx(mbar, gn.bytes);
         bulk_g2s(rawPcm, gn.src, gn.bytes, mbar);
       } else if (chunk + 1 < chunkEnd) {
         const ChunkCtx cn = load_chunk<F>(p, chunk + 1);
         sCx[cpar ^ 1] = cn;                           // read by everyone after the barriers of this tile
         const TileGeom gn = tile_geom<F>(p, cn, 0);
+        sTg[0] = gn.count; sTg[1] = gn.mis; sTg[2] = gn.lead;
         mbar_expect_tx(mbar, gn.bytes);
         bulk_g2s(rawPcm, gn.src, gn.bytes, mbar);
       }
@@ -393,7 +463,7 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
         p.out[(cx.row0 + tfs + ff) * p.outStride + p.outCol + c] = ring[c * (2 * F) + ringBase + ff];
       }
     } else {
-      const int K = p.nStat, W1 = p.fW1, W2 = p.fW2, H = W1 + W2;
+      const int K = KC ? KC : p.nStat, W1 = p.fW1, W2 = p.fW2, H = W1 + W2;
       const int T = cx.T;
       const int r0 = emitted;
       const int r1 = (j + 1 == cx.nT) ? cx.b : min(tfs + F - H, cx.b);
@@ -401,21 +471,38 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
       const float norm1 = p.fNorm1, norm2 = p.fNorm2;
       const int d0 = max(r0 - W2, 0), d1 = min(r1 + W2, T1);
       const int dRows = F + 24;
-      float *outS = Dbuf + ((K * dRows + 3) & ~3);
       const int K3 = 3 * K;
       const int nr = r1 - r0;
+      float *o = p.out + (cx.row0 + r0) * (long long)K3;
+      // the rows are staged at the global rows' offset modulo 16 bytes (the 3 floats of slack are behind Dbuf in the
+      // dead FFT tile), so that the store below moves them 16 bytes at a time
+      const int oMis = (int)((reinterpret_cast<uintptr_t>(o) >> 2) & 3);
+      float *outS = Dbuf + ((K * dRows + 3) & ~3) + oMis;
       const bool interior1 = (d0 >= W1) && (d1 + W1 <= T);
       const bool interior2 = (r0 >= W2) && (r1 <= c02);
       if (interior1 && interior2 && W1 == 2 && W2 == 2 && nr == F) {
-        emit_interior<F, NT>(ring, Dbuf, outS, K, dRows, d0 - cx.s0, r0 - cx.s0, norm1, p.fRcp1, norm2, p.fRcp2, tid);
+        if constexpr (KC != 0)
+          emit_interior_k<KC>(ring, Dbuf, outS, d0 - cx.s0, r0 - cx.s0, norm1, p.fRcp1, norm2, p.fRcp2, tid);
+        else
+          emit_interior<F, NT>(ring, Dbuf, outS, K, dRows, d0 - cx.s0, r0 - cx.s0, norm1, p.fRcp1, norm2, p.fRcp2, tid);
+      } else if (KC != 0 && W1 == 2 && W2 == 2) {
+        if constexpr (KC != 0)    // K and the windows at compile time: the window sums are straight-line code
+          emit_edge<F, NW, KC, 2>(ring, Dbuf, outS, K, W1, W2, T, T1, c01, c02, cx.s0, r0, r1, d0, d1, dRows, norm1, p.fRcp1, norm2, p.fRcp2, warp, f);
       } else {
         emit_edge<F, NW>(ring, Dbuf, outS, K, W1, W2, T, T1, c01, c02, cx.s0, r0, r1, d0, d1, dRows, norm1, p.fRcp1, norm2, p.fRcp2, warp, f);
       }
       OSM_PHASE(kPhEmit);
       {
-        float *o = p.out + (cx.row0 + r0) * (long long)K3;
+        // rows [r0, r1) are contiguous in p.out: up to 3 leading floats, 16-byte groups, up to 3 trailing floats
         const int n = nr * K3;
-        for (int i = tid; i < n; i += NT) o[i] = outS[i];
+        const int head = min((4 - oMis) & 3, n);
+        const int nv = (n - head) >> 2, tail = head + 4 * nv;
+        if (tid < head) o[tid] = outS[tid];
+        const float4 *sv = reinterpret_cast<const float4 *>(outS + head);
+        float4 *gv = reinterpret_cast<float4 *>(o + head);
+#pragma unroll 1
+        for (int i = tid; i < nv; i += NT) gv[i] = sv[i];
+        if (tid < n - tail) o[tail + tid] = outS[tail + tid];
       }
       emitted = r1;
     }
@@ -442,11 +529,11 @@ __global__ void __launch_bounds__(kNT, 2) lld512_kernel(const LldParams p)
 #endif
 }
 
-template <int NZR>
+template <int NZR, int KC>
 cudaError_t launch_fast_t(const LldParams &p, int numSMs, cudaStream_t st, LldLaunchInfo *info, bool launch)
 {
   const size_t smem = (size_t)make_layout(p, kM, kF).total;
-  auto kern = lld512_kernel<NZR>;
+  auto kern = lld512_kernel<NZR, KC>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   int occ = 0;
@@ -474,8 +561,13 @@ bool lld_fast_applies(const LldParams &p, int nfft)
 
 cudaError_t launch_lld_fast(const LldParams &p, int numSMs, cudaStream_t st, LldLaunchInfo *info, bool launch)
 {
-  if (p.frameSize <= 416) return launch_fast_t<13>(p, numSMs, st, info, launch);
-  return launch_fast_t<16>(p, numSMs, st, info, launch);
+  // 13 static columns (MFCC 0..12, the shipped MFCC12 sets) take the compile-time emission
+  if (p.frameSize <= 416) {
+    if (p.nStat == 13) return launch_fast_t<13, 13>(p, numSMs, st, info, launch);
+    return launch_fast_t<13, 0>(p, numSMs, st, info, launch);
+  }
+  if (p.nStat == 13) return launch_fast_t<16, 13>(p, numSMs, st, info, launch);
+  return launch_fast_t<16, 0>(p, numSMs, st, info, launch);
 }
 
 #ifdef OSM_LLD_PHASE_CLOCKS

@@ -1,7 +1,16 @@
-"""A/B timing of the cfg-2 fused kernel across library variants (opensmile_b200/variants/lib_*.so built with -D switches) and the
-default library: one subprocess per library (OSM_B200_LIB), 1 M frames device-resident, CUDA events over 20 launches after 5 warm-ups."""
+"""A/B timing of the cfg-2 fused kernel across library variants (opensmile_b200/variants/lib_*.so, e.g. the parent commit's
+library or builds with -D switches) and the default library: 1 M frames device-resident, CUDA events over 20 launches after
+5 warm-ups, one subprocess per library (OSM_B200_LIB) and round.  The libraries alternate round by round, so that a drift
+of the card's clock or of the neighbours' load over the run reaches every library alike.
+
+    python scripts/ab_lld512.py [--rounds R]       # default 5 rounds
+
+Prints every run (time, rate, checksum of the output rows) and per library the median, the range and the spread
+(max - min over median) of the per-launch times."""
+import argparse
 import glob
 import os
+import statistics
 import subprocess
 import sys
 
@@ -27,12 +36,39 @@ for _ in range(20):
 b.record()
 torch.cuda.synchronize()
 ms = a.elapsed_time(b) / 20
-print("%%.4f ms  %%.1f M frames/s  checksum %%.6e" %% (ms, out.shape[0] / ms / 1e3, float(out.double().abs().sum())))
+print("RESULT %%.4f %%.1f %%.6e" %% (ms, out.shape[0] / ms / 1e3, float(out.double().abs().sum())))
 ''' % ROOT
-libs = [("default", None)] + [(os.path.basename(p), p) for p in sorted(glob.glob(os.path.join(ROOT, "opensmile_b200", "variants", "lib_*.so")))]
-for name, path in libs:
-    env = dict(os.environ)
-    if path:
-        env["OSM_B200_LIB"] = path
-    r = subprocess.run([sys.executable, "-c", CHILD], env=env, capture_output=True, text=True)
-    print("%-28s %s" % (name, (r.stdout.strip().splitlines() or [r.stderr[-300:]])[-1]))
+
+
+def main(argv):
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--rounds", type=int, default=5)
+    args = ap.parse_args(argv)
+    libs = [("default", None)] + [(os.path.basename(p), p) for p in
+                                  sorted(glob.glob(os.path.join(ROOT, "opensmile_b200", "variants", "lib_*.so")))]
+    times = {name: [] for name, _ in libs}
+    sums = {name: set() for name, _ in libs}
+    for rnd in range(args.rounds):
+        order = libs if rnd % 2 == 0 else libs[::-1]
+        for name, path in order:
+            env = dict(os.environ)
+            if path:
+                env["OSM_B200_LIB"] = path
+            r = subprocess.run([sys.executable, "-c", CHILD], env=env, capture_output=True, text=True)
+            line = [s for s in r.stdout.splitlines() if s.startswith("RESULT ")]
+            if r.returncode != 0 or not line:
+                raise SystemExit("%s failed:\n%s" % (name, r.stderr[-2000:]))
+            ms, rate, chk = line[-1].split()[1:]
+            times[name].append(float(ms))
+            sums[name].add(chk)
+            print("round %d  %-28s %s ms  %s M frames/s  checksum %s" % (rnd, name, ms, rate, chk), flush=True)
+    print("\n%-28s %10s %10s %10s %8s  %s" % ("library", "median ms", "min", "max", "spread", "checksum"))
+    for name, _ in libs:
+        t = times[name]
+        med = statistics.median(t)
+        print("%-28s %10.4f %10.4f %10.4f %7.2f%%  %s" % (name, med, min(t), max(t), 100 * (max(t) - min(t)) / med,
+                                                        " ".join(sorted(sums[name]))))
+
+
+if __name__ == "__main__":
+    main(sys.argv[1:])
