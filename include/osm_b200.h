@@ -141,9 +141,18 @@ typedef struct {            /* cWaveSource (src/iocore/waveSource.cpp) */
 typedef struct {            /* cFramer */
   double  frameSize;        /* 0.025 */
   double  frameStep;        /* 0 = frameSize */
-  int32_t frameCenterSpecialLeft; /* 1 (only `left` is supported) */
+  /* sampling centre (core/winToVecProcessor.cpp:461-508): frameCenterSpecial, when set, overrides the other two;
+   * frameCenterFrames, when set, overrides frameCenter */
+  int32_t frameCenterSpecial;     /* osm_b200_frame_center, OSM_B200_CENTER_UNSET */
+  int32_t frameCenterFramesSet;   /* 0 */
+  double  frameCenter;            /* 0 (seconds) */
+  int32_t frameCenterFrames;      /* 0 (samples), read when frameCenterFramesSet */
   int32_t noPostEOIprocessing;    /* 1 */
 } osm_b200_framer;
+
+/* cFramer.frameCenterSpecial: the first two letters of the value, case-insensitive ("mi" / "ce" = frame centre,
+ * "ri" = frame end, anything else = frame start) */
+typedef enum { OSM_B200_CENTER_UNSET = 0, OSM_B200_CENTER_LEFT = 1, OSM_B200_CENTER_MID = 2, OSM_B200_CENTER_RIGHT = 3 } osm_b200_frame_center;
 
 typedef struct { double k; int32_t de; } osm_b200_vectorpreemphasis;  /* 0.97, 0 */
 

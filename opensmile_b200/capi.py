@@ -54,8 +54,8 @@ class WaveSource(C.Structure):
 
 
 class Framer(C.Structure):
-    _fields_ = [("frameSize", f64), ("frameStep", f64), ("frameCenterSpecialLeft", i32),
-                ("noPostEOIprocessing", i32)]
+    _fields_ = [("frameSize", f64), ("frameStep", f64), ("frameCenterSpecial", i32), ("frameCenterFramesSet", i32),
+                ("frameCenter", f64), ("frameCenterFrames", i32), ("noPostEOIprocessing", i32)]
 
 
 class VectorPreemphasis(C.Structure):

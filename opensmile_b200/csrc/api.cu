@@ -235,7 +235,7 @@ osm_b200_status osm_b200_component_defaults(int32_t type, osm_b200_component *c)
       break;
     case OSM_B200_C_FRAMER:
       c->u.framer.frameSize = 0.025; c->u.framer.frameStep = 0.0;
-      c->u.framer.frameCenterSpecialLeft = 1; c->u.framer.noPostEOIprocessing = 1;
+      c->u.framer.frameCenterSpecial = OSM_B200_CENTER_UNSET; c->u.framer.noPostEOIprocessing = 1;
       break;
     case OSM_B200_C_VECTORPREEMPHASIS: c->u.vectorpreemphasis.k = 0.97; c->u.vectorpreemphasis.de = 0; break;
     case OSM_B200_C_WINDOWER:
@@ -377,7 +377,7 @@ static osm_b200_status build_pass(osm_b200_plan *pl, int si, int opIdx, bool dum
   memset(&kp, 0, sizeof kp);
   kp.opKind = -1;
   kp.nChan = kernel_nchan(fe); kp.pcmF32 = fe.format != OSM_B200_PCM_S16;
-  kp.frameSize = fe.frameSize; kp.frameStep = fe.frameStep;
+  kp.frameSize = fe.frameSize; kp.frameStep = fe.frameStep; kp.frameCenter = fe.frameCenter;
   kp.hopMagic = (unsigned)((0x100000000ull + (unsigned long long)fe.frameStep - 1) / (unsigned long long)fe.frameStep);
   // per-lane stride S = frameStep + sPad of the shared-memory sample tile: odd S (scalar loads)
   // or even S with S/2 odd (64-bit sample-pair loads) is bank-conflict free across the lanes
@@ -527,7 +527,7 @@ static osm_b200_status build_pass(osm_b200_plan *pl, int si, int opIdx, bool dum
         kp.plpAud = 0; kp.plpInvLog = 0; kp.plpIDFT = 0; kp.plpLP = 0; kp.plpCeps = 0; kp.plpLifter = 0;
         kp.nStat = kp.nBands;
         memset(&pr.rp, 0, sizeof pr.rp);
-        pr.rp.nBands = kp.nBands; pr.rp.frameSize = fe.frameSize; pr.rp.frameStep = fe.frameStep;
+        pr.rp.nBands = kp.nBands; pr.rp.frameSize = fe.frameSize; pr.rp.frameStep = fe.frameStep; pr.rp.frameCenter = fe.frameCenter;
         pr.rp.mode = op.plp.rasta; pr.rp.iir = op.plp.rastaIir;
         for (int i = 0; i < 5; i++) pr.rp.fir[i] = op.plp.rastaFir[i];
       }
@@ -575,15 +575,18 @@ static osm_b200_status build_groups(osm_b200_plan *pl, bool simple, int &seqLagD
         if (segCols > 32) return fail(OSM_B200_ERR_UNSUPPORTED, "cDeltaRegression(onlyInSegments): more than 32 elements");
       }
       if (G.segId >= kMaxSegIds) return fail(OSM_B200_ERR_UNSUPPORTED, "too many onlyInSegments delta components");
-      sq.frameSize = d.streams[g.stream].fe.frameSize; sq.frameStep = d.streams[g.stream].fe.frameStep;
+      sq.frameSize = d.streams[g.stream].fe.frameSize; sq.frameStep = d.streams[g.stream].fe.frameStep; sq.frameCenter = d.streams[g.stream].fe.frameCenter;
       continue;
     }
     if (pp.nGroups >= kMaxPostGroups) return fail(OSM_B200_ERR_UNSUPPORTED, "too many output groups");
     PostGroup &pg = pp.groups[pp.nGroups++];
     pg.srcCol = g.srcCol; pg.n = g.n; pg.outCol = g.outCol; pg.nStages = (int)g.stages.size();
-    pg.frameSize = d.streams[g.stream].fe.frameSize; pg.frameStep = d.streams[g.stream].fe.frameStep;
+    pg.frameSize = d.streams[g.stream].fe.frameSize; pg.frameStep = d.streams[g.stream].fe.frameStep; pg.frameCenter = d.streams[g.stream].fe.frameCenter;
     pg.nLim = 0;
-    for (int ls : g.limitStreams) if (pg.nLim < 3) { pg.limSize[pg.nLim] = d.streams[ls].fe.frameSize; pg.limStep[pg.nLim] = d.streams[ls].fe.frameStep; pg.nLim++; }
+    for (int ls : g.limitStreams) if (pg.nLim < 3) {
+      pg.limSize[pg.nLim] = d.streams[ls].fe.frameSize; pg.limStep[pg.nLim] = d.streams[ls].fe.frameStep; pg.limCenter[pg.nLim] = d.streams[ls].fe.frameCenter;
+      pg.nLim++;
+    }
     for (size_t i = 0; i < g.stages.size(); i++) { pg.kind[i] = g.stages[i].kind; pg.win[i] = g.stages[i].win; pg.flags[i] = g.stages[i].flags; if (g.stages[i].kind == ST_CMS) pl->needMeans = true; }
   }
   pp.nStat = d.nStatic; pp.maxN = 1; pp.halo = 0;
@@ -722,7 +725,7 @@ static osm_b200_status build_shs_chain(const PlanDesc &d, const StaticOp &op, co
     return fail(OSM_B200_ERR_UNSUPPORTED, "cSpecScale: spectrum too long for the SHS kernel's workspace");
   ViterbiParams &vp = rt.vit;
   memset(&vp, 0, sizeof vp);
-  vp.nShsCols = pc.nShsCols; vp.nCand = pc.nCand; vp.frameSize = fe.frameSize; vp.frameStep = fe.frameStep;
+  vp.nShsCols = pc.nShsCols; vp.nCand = pc.nCand; vp.frameSize = fe.frameSize; vp.frameStep = fe.frameStep; vp.frameCenter = fe.frameCenter;
   vp.statStride = d.nStatic; vp.outCol = op.outCol; vp.bufLen = pc.bufLen;
   vp.oF0final = pc.oF0final; vp.oF0finalLog = pc.oF0finalLog; vp.oF0finalEnv = pc.oF0finalEnv; vp.oF0finalEnvLog = pc.oF0finalEnvLog;
   vp.oVClipped = pc.oVClipped; vp.oVUnclipped = pc.oVUnclipped;
@@ -738,7 +741,7 @@ static osm_b200_status build_jitter(const PlanDesc &d, const StaticOp &op, const
   const JitterOp &jo = op.jitter;
   JitterParams &jp = rt.jit;
   memset(&jp, 0, sizeof jp);
-  jp.nChan = kernel_nchan(fe); jp.pcmF32 = fe.format != OSM_B200_PCM_S16; jp.frameSize = fe.frameSize; jp.frameStep = fe.frameStep;
+  jp.nChan = kernel_nchan(fe); jp.pcmF32 = fe.format != OSM_B200_PCM_S16; jp.frameSize = fe.frameSize; jp.frameStep = fe.frameStep; jp.frameCenter = fe.frameCenter;
   jp.Ts = 1.0 / fe.sampleRate;                               // period of the wave level
   jp.pitchT = fe.frameStepSec;                               // period of the F0 level (core/winToVecProcessor.cpp:563)
   jp.statStride = d.nStatic; jp.f0Col = d.ops[jo.pitchOp].outCol + jo.f0Col; jp.outCol = op.outCol;
@@ -785,7 +788,7 @@ static osm_b200_status build_acf_pitch(const PlanDesc &d, const StaticOp &op, co
   ap.maxPitch = po.maxPitch; ap.voicingCutoff = po.voicingCutoff; ap.fsSec = po.fsSec;
   ap.voiceProb = po.voiceProb; ap.voiceQual = po.voiceQual; ap.HNR = po.HNR; ap.HNRdB = po.HNRdB; ap.linHNR = po.linHNR;
   ap.F0 = po.F0; ap.F0raw = po.F0raw; ap.F0env = po.F0env;
-  ap.statStride = d.nStatic; ap.outCol = op.outCol; ap.frameSize = fe.frameSize; ap.frameStep = fe.frameStep;
+  ap.statStride = d.nStatic; ap.outCol = op.outCol; ap.frameSize = fe.frameSize; ap.frameStep = fe.frameStep; ap.frameCenter = fe.frameCenter;
   // complex FFT of size nfft: same factorisation tables as lld_kernel's M = nfft, plus one spare entry (zero)
   std::vector<float2> tw;
   build_twiddles(fe.nfft, tw, ap.twOff);
@@ -802,7 +805,7 @@ static osm_b200_status build_time_op(const PlanDesc &d, const StaticOp &op, cons
   TimeOpParams &tp = rt.tp;
   memset(&tp, 0, sizeof tp);
   tp.nChan = kernel_nchan(fe); tp.pcmF32 = fe.format != OSM_B200_PCM_S16; tp.F = srt.tileF; tp.statStride = d.nStatic; tp.outCol = op.outCol;
-  tp.frameSize = fe.frameSize; tp.frameStep = fe.frameStep;
+  tp.frameSize = fe.frameSize; tp.frameStep = fe.frameStep; tp.frameCenter = fe.frameCenter;
   tp.windowed = op.windowed; tp.preemph = op.windowed && fe.preemph; tp.preDe = fe.preDe; tp.preK = fe.preK;
   tp.oneMinusK = 1 - fe.preK; tp.winOffset = fe.winOffset; tp.window = srt.dWindow;
   if (op.kind == SOP_INTENSITY) {
@@ -981,7 +984,14 @@ double osm_b200_plan_row_time(const osm_b200_plan *pl, int64_t r)
 {
   if (!pl) return 0.0;
   const FrontEnd &fe = pl->d.fe0();
-  return fe.rowSampleStep > 0 ? (double)(r * fe.rowSampleStep) * (1.0 / fe.sampleRate) : (double)r * fe.frameStepSec;
+  if (fe.rowSampleStep > 0) return (double)(r * fe.rowSampleStep) * (1.0 / fe.sampleRate);
+  if (fe.frameCenter == 0 && fe.timeOffset == 0.0) return (double)r * fe.frameStepSec;
+  // a centred frame carries the time of its first sample read (clamped at the input start) + frameCenter
+  // (core/winToVecProcessor.cpp:1076-1079, core/dataMemoryLevel.cpp:1651-1697); a time of exactly 0 is replaced by
+  // r * frame period when the frame is written (core/dataMemoryLevel.cpp:1211-1212), which `right` gives its padded frames
+  const long long s0 = frame_first_sample(r, fe.frameStep, fe.frameCenter);
+  const double t = (double)(s0 > 0 ? s0 : 0) * (1.0 / fe.sampleRate) + fe.timeOffset;
+  return t == 0.0 ? (double)r * fe.frameStepSec : t;
 }
 int32_t osm_b200_plan_frame_size_samples(const osm_b200_plan *pl) { return pl ? pl->d.fe0().frameSize : 0; }
 int32_t osm_b200_plan_frame_step_samples(const osm_b200_plan *pl) { return pl ? pl->d.fe0().frameStep : 0; }

@@ -55,7 +55,7 @@ __global__ void __launch_bounds__(kFmtThreads) formant_kernel(const FormantParam
       float *planes = xw;                                        // [kFmtWarps][4][kPlane]: in / out, real / imaginary
       const float *wc = p.D, *cosT = p.D + ro::kNw + ro::kNc, *sinT = cosT + (size_t)p.kHalf * IP;
       for (int f = 0; f < nb; f++) {
-        FrameReader<F32> fr{tp, tp.pcm + (uo + (long long)(tl.f0 + fb + f) * tp.frameStep) * tp.nChan};
+        FrameReader<F32> fr{tp, tp.pcm + uo * tp.nChan, frame_first_sample(tl.f0 + fb + f, tp.frameStep, tp.frameCenter)};
         float *re = planes + (size_t)f * 4 * ro::kPlane, *im = re + ro::kPlane;
         for (int n = tid; n < ro::kN; n += kFmtThreads) {
           const int m = n - p.padLeft;
@@ -134,7 +134,7 @@ __global__ void __launch_bounds__(kFmtThreads) formant_kernel(const FormantParam
     } else {
     // 1. windowed frames (dspcore/windower.cpp:226) into shared memory
     for (int f = 0; f < nb; f++) {
-      FrameReader<F32> fr{tp, tp.pcm + (uo + (long long)(tl.f0 + fb + f) * tp.frameStep) * tp.nChan};
+      FrameReader<F32> fr{tp, tp.pcm + uo * tp.nChan, frame_first_sample(tl.f0 + fb + f, tp.frameStep, tp.frameCenter)};
       for (int m = tid; m < N; m += kFmtThreads) xw[f * N + m] = fr.at(m);
     }
     __syncthreads();

@@ -31,8 +31,10 @@ __device__ __forceinline__ float td_pcm(const TimeOpParams &p, const int16_t *s)
 template <bool F32>
 struct FrameReader {
   const TimeOpParams &p;
-  const int16_t *base;     // first sample frame of this frame
-  __device__ __forceinline__ float raw(int n) const { return td_pcm<F32>(p, base + (long long)n * p.nChan); }
+  const int16_t *utt;      // first sample frame of the utterance
+  long long s0;            // first sample of this frame within the utterance, frame_first_sample (< 0: a centred frame's padding)
+  // positions before the utterance start read its sample 0 (frame_geom.cuh)
+  __device__ __forceinline__ float raw(int n) const { return td_pcm<F32>(p, utt + max(s0 + n, 0LL) * p.nChan); }
   // the cVectorPreemphasis level (the framer level when p.preemph = 0)
   __device__ __forceinline__ float pre(int n) const
   {

@@ -80,11 +80,11 @@ __global__ void __launch_bounds__(kPostThreads) post_kernel(const PostParams p)
   for (int gi = 0; gi < p.nGroups; gi++) {
     const PostGroup &g = p.groups[gi];
     const int n = g.n;
-    const int T = (Ls >= g.frameSize) ? (int)((Ls - g.frameSize) / g.frameStep + 1) : 0;   // frames of this group's source level
+    const int T = (int)frame_count(Ls, g.frameSize, g.frameStep, g.frameCenter);   // frames of this group's source level
     // a multi-level reader delivers min over its levels: that bounds how many frames the first stage
     // produces (before EOI and in total), while reads of THIS level still clamp at its own end
     int Tlim = T;
-    for (int k = 0; k < g.nLim; k++) Tlim = min(Tlim, (Ls >= g.limSize[k]) ? (int)((Ls - g.limSize[k]) / g.limStep[k] + 1) : 0);
+    for (int k = 0; k < g.nLim; k++) Tlim = min(Tlim, (int)frame_count(Ls, g.limSize[k], g.limStep[k], g.limCenter[k]));
     // level 0 view of this group: copy its columns so that every level has row stride n
     const float *cur;
     {
@@ -365,7 +365,7 @@ __global__ void pitch_smooth_kernel(const AcfPitchParams p, int u0, int u1)
   const int u = u0 + blockIdx.x * blockDim.x + threadIdx.x;
   if (u >= u1) return;
   const long long Ls = p.uttOff[u + 1] - p.uttOff[u];
-  const int T = (Ls >= p.frameSize) ? (int)((Ls - p.frameSize) / p.frameStep + 1) : 0;
+  const int T = (int)frame_count(Ls, p.frameSize, p.frameStep, p.frameCenter);
   const int n = p.nfft / 2;
   const double Tsamp = (double)p.fsSec / (double)(2 * n);
   float lastPitch = 0.f, lastlastPitch = 0.f, glMeanPitch = 0.f, pitchEnv = 0.f;
@@ -503,7 +503,7 @@ __global__ void rasta_kernel(const RastaParams p, int u0, int u1)
   const int u = u0 + (int)(idx / nB), b = (int)(idx % nB);
   if (u >= u1) return;
   const long long L = p.uttOff[u + 1] - p.uttOff[u];
-  const long long T = (L < p.frameSize) ? 0 : (L - p.frameSize) / p.frameStep + 1;
+  const long long T = frame_count(L, p.frameSize, p.frameStep, p.frameCenter);
   float *x = p.band + p.statOff[u] * nB + b;
   if (p.mode == 1) {
     float fir[5] = {0.f, 0.f, 0.f, 0.f, 0.f};   // circular input history, slot ptr = newest
@@ -608,8 +608,8 @@ __global__ void cms_mean_kernel(const PostParams p, float *means, int u0, int u1
   for (int gi = 0; gi < p.nGroups; gi++) {
     const PostGroup &g = p.groups[gi];
     if (g.nStages < 1 || g.kind[g.nStages - 1] != 2) continue;
-    int T = (Ls >= g.frameSize) ? (int)((Ls - g.frameSize) / g.frameStep + 1) : 0;
-    for (int k = 0; k < g.nLim; k++) T = min(T, (Ls >= g.limSize[k]) ? (int)((Ls - g.limSize[k]) / g.limStep[k] + 1) : 0);
+    int T = (int)frame_count(Ls, g.frameSize, g.frameStep, g.frameCenter);
+    for (int k = 0; k < g.nLim; k++) T = min(T, (int)frame_count(Ls, g.limSize[k], g.limStep[k], g.limCenter[k]));
     for (int c = threadIdx.x; c < g.n; c += blockDim.x) {
       float m = 0.f;
       if (T > 0) {

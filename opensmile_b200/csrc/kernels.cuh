@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 
+#include "frame_geom.cuh"
+
 namespace osm {
 
 constexpr int kMaxVW = 32;   // virtual warps (F-lane groups) per CTA
@@ -81,21 +83,23 @@ struct LldParams {
   // toneSqrt = usePower; chromaOct > 0 folds the notes into that many chroma values, 0 outputs the notes
   int toneSqrt, chromaOct;
   float chromaSilThresh;
+  // ---- front end (cont.) ----
+  int frameCenter;               // frame t starts at sample t * frameStep - frameCenter of its utterance (frame_geom.cuh)
 };
 
 // temporal post-processing (cDeltaRegression / cContourSmoother chains)
 struct PostGroup {
   int srcCol, n, outCol;
-  int frameSize, frameStep;      // geometry of the stream the source level belongs to (defines its T)
+  int frameSize, frameStep, frameCenter;   // geometry of the stream the source level belongs to (defines its T)
   // the source sits in a multi-level reader / concat together with levels of other streams: the
   // reader only delivers min over them (core/dataReader.cpp:375-380) -> T = min(T, T of these)
-  int nLim; int limSize[3], limStep[3];
+  int nLim; int limSize[3], limStep[3], limCenter[3];
   int nStages;
   int kind[3];                   // 0 = delta, 1 = sma, 2 = utterance mean subtraction (cFullinputMean)
   int win[3];
   int flags[3];
 };
-constexpr int kMaxPostGroups = 16;
+constexpr int kMaxPostGroups = 24;   // emo_large.conf: 6 smoothed levels x (sma, Δ, ΔΔ) = 18
 struct PostParams {
   const float *stat;             // static rows
   int statStride;
@@ -166,7 +170,7 @@ struct TimeOpParams {            // cEnergy / cMZcr on the framer or windower le
   const long long *uttOff, *statOff;
   const OpTile *tiles; int nTiles; int F;
   float *stat; int statStride, outCol;
-  int frameSize, frameStep;
+  int frameSize, frameStep, frameCenter;
   int windowed, preemph, preDe; float preK, oneMinusK, winOffset;
   const float *window;           // [frameSize] (device), only when windowed
   // cEnergy
@@ -194,7 +198,7 @@ struct AcfPitchParams {
   int voiceProb, voiceQual, HNR, HNRdB, linHNR, F0, F0raw, F0env;
   // smoothing pass
   float *stat; int statStride, outCol;
-  int frameSize, frameStep, nUtt;
+  int frameSize, frameStep, frameCenter, nUtt;
 };
 cudaError_t launch_acf_pitch(const AcfPitchParams &p, cudaStream_t st);     // per-frame analysis -> raw
 cudaError_t launch_pitch_smooth(const AcfPitchParams &p, int u0, int u1, cudaStream_t st);   // raw -> static columns
@@ -206,7 +210,7 @@ bool acf_pitch_supported_fft(int nfft);
 struct RastaParams {
   float *band; int nBands;       // [static rows][nBands]
   const long long *uttOff, *statOff;
-  int frameSize, frameStep;
+  int frameSize, frameStep, frameCenter;
   int mode;                      // 1 RASTA, 2 newRASTA
   float fir[5], iir;
 };
@@ -321,7 +325,7 @@ cudaError_t launch_shs(const ShsParams &p, cudaStream_t st);
 struct ViterbiParams {
   const float *shs; int nShsCols, nCand;
   const long long *uttOff, *statOff;
-  int frameSize, frameStep;
+  int frameSize, frameStep, frameCenter;
   float *stat; int statStride, outCol;
   int *lag;                      // [nUtt] frames the level holds before the end-of-input flush
   int bufLen;
@@ -335,7 +339,7 @@ cudaError_t launch_viterbi(const ViterbiParams &p, int u0, int u1, cudaStream_t 
 struct JitterParams {
   const int16_t *pcm; int nChan; int pcmF32;   // pcmF32: see LldParams
   const long long *uttOff, *statOff;
-  int frameSize, frameStep;
+  int frameSize, frameStep, frameCenter;
   double Ts, pitchT;             // wave sample period, period of the F0 level
   float *stat; int statStride, f0Col, outCol;
   double searchRangeRel; float threshCC, lgHNRfloor; int minNumPeriods;
@@ -357,7 +361,7 @@ struct SeqPostParams {
   const long long *statOff, *rowOff, *uttOff;
   float *out; int outStride;
   const int *lag;
-  int frameSize, frameStep;
+  int frameSize, frameStep, frameCenter;
   int nGroups;
   SeqGroup groups[kMaxSeqGroups];
 };

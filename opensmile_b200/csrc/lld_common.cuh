@@ -134,7 +134,10 @@ struct ChunkCtx {
   long long row0;    // output row of frame 0 of the utterance
 };
 
-template <int F>
+// CENTRED: frames start at t * frameStep - LldParams::frameCenter (lld_kernel).  Without it the left-framed geometry alone
+// (frame_geom.cuh with centre 0) is compiled, in the form lld512_kernel's instruction stream was tuned on; lld512_kernel never
+// serves a centred stream (lld_fast_applies).
+template <int F, bool CENTRED = false>
 __device__ __forceinline__ ChunkCtx load_chunk(const LldParams &p, int chunk)
 {
   ChunkCtx c;
@@ -142,7 +145,8 @@ __device__ __forceinline__ ChunkCtx load_chunk(const LldParams &p, int chunk)
   c.utt = cr.utt; c.a = cr.a; c.b = cr.b; c.tile0 = cr.tile0;
   c.uo = p.uttOff[cr.utt];
   const long long Ls = p.uttOff[cr.utt + 1] - c.uo;
-  c.T = (int)((Ls - p.frameSize) / p.frameStep + 1);
+  if constexpr (CENTRED) c.T = (int)frame_count(Ls, p.frameSize, p.frameStep, p.frameCenter);
+  else c.T = (int)((Ls - p.frameSize) / p.frameStep + 1);
   c.s0 = max(cr.a - p.halo, 0);
   c.sEnd = min(cr.b + p.halo, c.T);
   c.nT = (c.sEnd - c.s0 + F - 1) / F;
@@ -169,25 +173,55 @@ struct TileGeom {
   int nf;            // frames in this tile
   int count;         // sample frames the tile covers
   int lead;          // sample frames fetched before the tile start (0 at the utterance start)
+  int pad;           // centred frames: sample frames of the tile before the utterance start (copies of its sample 0, not fetched)
   int mis;           // bytes between the 16-byte aligned fetch address and the first wanted byte
   uint32_t bytes;    // bulk copy size
   const char *src;   // 16-byte aligned fetch address
 };
 
-template <int F>
+// CENTRED (see load_chunk): the fetch stays inside the tile's utterance -- a tile whose first frames start before it fetches
+// from its sample 0 on (pad > 0), and the lead frames stop at its start.
+template <int F, bool CENTRED = false>
 __device__ __forceinline__ TileGeom tile_geom(const LldParams &p, const ChunkCtx &c, int j)
 {
   TileGeom g;
   g.fs = c.s0 + j * F;
   g.nf = min(F, c.sEnd - g.fs);
-  const long long s0 = (long long)g.fs * p.frameStep;
   g.count = (g.nf - 1) * p.frameStep + p.frameSize;
-  g.lead = (s0 > 0) ? kLeadFrames : 0;
-  const char *a = reinterpret_cast<const char *>(p.pcm + (c.uo + s0 - g.lead) * p.nChan);
+  const char *a;
+  if constexpr (CENTRED) {
+    const long long s0 = frame_first_sample(g.fs, p.frameStep, p.frameCenter);
+    g.pad = s0 < 0 ? (int)-s0 : 0;
+    g.lead = (int)min(max(s0, 0LL), (long long)kLeadFrames);
+    a = reinterpret_cast<const char *>(p.pcm + (c.uo + s0 + g.pad - g.lead) * p.nChan);
+  } else {
+    const long long s0 = (long long)g.fs * p.frameStep;
+    g.pad = 0;
+    g.lead = (s0 > 0) ? kLeadFrames : 0;
+    a = reinterpret_cast<const char *>(p.pcm + (c.uo + s0 - g.lead) * p.nChan);
+  }
   g.mis = (int)(reinterpret_cast<uintptr_t>(a) & 15);
   g.src = a - g.mis;
-  g.bytes = (uint32_t)align_up(g.mis + (g.lead + g.count) * p.nChan * 2, 16);
+  g.bytes = (uint32_t)align_up(g.mis + (g.lead + g.count - g.pad) * p.nChan * 2, 16);
   return g;
+}
+
+// Staging of a tile whose first frames start before the utterance (centred framing, first tile(s) of an utterance only):
+// tile sample i is utterance sample max(i - pad, 0); rp = utterance sample 0 in the landing zone.  Same conversion,
+// pre-emphasis and layout as the staging loop of lld_kernel; ks = the signed pre-emphasis coefficient, 0 without pre-emphasis.
+// (Scalars, not the LldParams block: a reference to it would make the caller copy the block to its stack.)
+template <int F, int NT, bool F32>
+__device__ OSM_COLD void stage_padded_tile(const int16_t *rp, int pad, int count, int hop, int sPad, int nChan, float ks,
+                                           float *samp, float *raw, int tid)
+{
+  for (int i = tid; i < count; i += NT) {
+    const float x = pcm_to_float_slow<F32>(rp + max(i - pad, 0) * nChan, nChan);
+    float y = x;
+    if (ks != 0.f && i > 0) y = __fadd_rn(x, __fmul_rn(ks, pcm_to_float_slow<F32>(rp + max(i - 1 - pad, 0) * nChan, nChan)));
+    const int q = i / hop, r = i - q * hop;
+    if (r == 0 && q < F) raw[q] = x;
+    samp[i + q * sPad] = y;
+  }
 }
 
 // x / d.  rcp != 0 marks a divisor (2, 10, 28, 60 = the delta norms of windows 1..4) for which the

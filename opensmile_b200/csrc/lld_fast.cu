@@ -555,7 +555,7 @@ cudaError_t launch_fast_t(const LldParams &p, int numSMs, cudaStream_t st, LldLa
 bool lld_fast_applies(const LldParams &p, int nfft)
 {
   return nfft == 512 && !p.narrow && p.opKind == 0 && p.magOut == nullptr && p.melUsePower && p.nChan == 1 &&
-         p.frameStep % 8 == 0 && p.frameSize % 8 == 0 && p.frameSize <= 512 && !p.hasWinOffset && p.nStat <= kKMax &&
+         p.frameCenter == 0 && p.frameStep % 8 == 0 && p.frameSize % 8 == 0 && p.frameSize <= 512 && !p.hasWinOffset && p.nStat <= kKMax &&
          ((p.frameStep + p.sPad) % 2) == 0;
 }
 

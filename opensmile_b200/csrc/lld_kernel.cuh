@@ -36,7 +36,8 @@ namespace osm {
 // GEN = false: the MFCC-only instance (band op = cMfcc, no magnitude level dump); the PLP back end and
 // the magnitude dump compile away.  GEN = true: band op and dump selected at run time.
 // F32: the instance for pre-converted mono float samples (LldParams::pcmF32).
-template <int M, int F, int NT, int MINB, bool VEC2, bool GEN, bool F32>
+// CENTRED: the GEN instance for a centred framer (LldParams::frameCenter != 0), whose first tiles start before the utterance.
+template <int M, int F, int NT, int MINB, bool VEC2, bool GEN, bool F32, bool CENTRED = false>
 __global__ void __launch_bounds__(NT, MINB) lld_kernel(const LldParams p)
 {
   const int opKind = GEN ? p.opKind : 0;
@@ -101,17 +102,17 @@ __global__ void __launch_bounds__(NT, MINB) lld_kernel(const LldParams p)
   int chunk = sRun[0];
   const int chunkEnd = sRun[1];
   if (chunk >= chunkEnd) return;
-  ChunkCtx cx = load_chunk<F>(p, chunk);
+  ChunkCtx cx = load_chunk<F, CENTRED>(p, chunk);
   int j = 0;
   int emitted = cx.a;                 // next output row of the current chunk to be written
   if (tid == 0) {
-    const TileGeom g0 = tile_geom<F>(p, cx, 0);
+    const TileGeom g0 = tile_geom<F, CENTRED>(p, cx, 0);
     mbar_expect_tx(mbar, g0.bytes);
     bulk_g2s(rawPcm, g0.src, g0.bytes, mbar);
   }
 
   while (chunk < chunkEnd) {
-    const TileGeom tg = tile_geom<F>(p, cx, j);
+    const TileGeom tg = tile_geom<F, CENTRED>(p, cx, j);
     const int nf = tg.nf, count = tg.count;
 
     // ================= stage: PCM (smem, prefetched by the bulk copy) -> float -> pre-emphasis -> smem =================
@@ -121,7 +122,8 @@ __global__ void __launch_bounds__(NT, MINB) lld_kernel(const LldParams p)
       const int16_t *rp = reinterpret_cast<const int16_t *>(rawPcm + tg.mis) + tg.lead * nChan;   // sample frame 0 of the tile
       const bool fastLoad = (tg.mis == 0) && (nChan <= 2) && !F32;
       const bool fastStore = (p.sPad == 0) || (hop % 8 == 0);
-      for (int c = tid; c * 8 < count; c += NT) {
+      if (CENTRED && tg.pad > 0) stage_padded_tile<F, NT, F32>(rp, tg.pad, count, hop, p.sPad, nChan, p.preemph ? (p.preDe ? p.preK : -p.preK) : 0.f, samp, raw, tid);
+      else for (int c = tid; c * 8 < count; c += NT) {
         const int i = c * 8;
         const int nvalid = min(8, count - i);
         float x[8];
@@ -191,12 +193,12 @@ __global__ void __launch_bounds__(NT, MINB) lld_kernel(const LldParams p)
     // the landing zone is free again: fetch the next tile's PCM while this one is processed
     if (tid == 0) {
       if (j + 1 < cx.nT) {
-        const TileGeom gn = tile_geom<F>(p, cx, j + 1);
+        const TileGeom gn = tile_geom<F, CENTRED>(p, cx, j + 1);
         mbar_expect_tx(mbar, gn.bytes);
         bulk_g2s(rawPcm, gn.src, gn.bytes, mbar);
       } else if (chunk + 1 < chunkEnd) {
-        const ChunkCtx cn = load_chunk<F>(p, chunk + 1);
-        const TileGeom gn = tile_geom<F>(p, cn, 0);
+        const ChunkCtx cn = load_chunk<F, CENTRED>(p, chunk + 1);
+        const TileGeom gn = tile_geom<F, CENTRED>(p, cn, 0);
         mbar_expect_tx(mbar, gn.bytes);
         bulk_g2s(rawPcm, gn.src, gn.bytes, mbar);
       }
@@ -422,7 +424,7 @@ __global__ void __launch_bounds__(NT, MINB) lld_kernel(const LldParams p)
     if (j == cx.nT) {
       chunk++;
       j = 0;
-      if (chunk < chunkEnd) { cx = load_chunk<F>(p, chunk); emitted = cx.a; }
+      if (chunk < chunkEnd) { cx = load_chunk<F, CENTRED>(p, chunk); emitted = cx.a; }
     }
   }
 }
@@ -430,21 +432,21 @@ __global__ void __launch_bounds__(NT, MINB) lld_kernel(const LldParams p)
 // ------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------
-// "lld_kernel<M,F,NT,MINB,VEC2|SCALAR,GEN|MFCC>" ("lld_kernel_f32<...>" for float input), built once per instance
-template <int M, int F, int NT, int MINB, bool VEC2, bool GEN, bool F32>
+// "lld_kernel<M,F,NT,MINB,VEC2|SCALAR,GEN|MFCC|CENTRED>" ("lld_kernel_f32<...>" for float input), built once per instance
+template <int M, int F, int NT, int MINB, bool VEC2, bool GEN, bool F32, bool CENTRED>
 static const char *lld_kernel_name()
 {
   static const std::string name = std::string(F32 ? "lld_kernel_f32" : "lld_kernel") + "<" + std::to_string(M) + "," + std::to_string(F) + "," +
                                   std::to_string(NT) + "," + std::to_string(MINB) + (VEC2 ? ",VEC2" : ",SCALAR") +
-                                  (GEN ? ",GEN>" : ",MFCC>");
+                                  (CENTRED ? ",CENTRED>" : GEN ? ",GEN>" : ",MFCC>");
   return name.c_str();
 }
 
-template <int M, int F, int NT, int MINB, bool VEC2, bool GEN, bool F32>
+template <int M, int F, int NT, int MINB, bool VEC2, bool GEN, bool F32, bool CENTRED = false>
 static cudaError_t launch_g(const LldParams &p, int numSMs, cudaStream_t st, LldLaunchInfo *info, bool launch)
 {
   const size_t smem = (size_t)make_layout(p, M, F).total;
-  auto kern = lld_kernel<M, F, NT, MINB, VEC2, GEN, F32>;
+  auto kern = lld_kernel<M, F, NT, MINB, VEC2, GEN, F32, CENTRED>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   int occ = 0;
@@ -454,7 +456,7 @@ static cudaError_t launch_g(const LldParams &p, int numSMs, cudaStream_t st, Lld
   const int grid = launch ? p.nRuns : numSMs * occ;
   if (info) {
     info->grid = grid; info->block = NT; info->smem = smem; info->nChunks = p.nChunks;
-    info->kernel = lld_kernel_name<M, F, NT, MINB, VEC2, GEN, F32>();
+    info->kernel = lld_kernel_name<M, F, NT, MINB, VEC2, GEN, F32, CENTRED>();
   }
   if (!launch) return cudaSuccess;
   kern<<<grid, NT, smem, st>>>(p);
@@ -464,6 +466,7 @@ static cudaError_t launch_g(const LldParams &p, int numSMs, cudaStream_t st, Lld
 template <int M, int F, int NT, int MINB, bool VEC2, bool F32>
 static cudaError_t launch_t(const LldParams &p, int numSMs, cudaStream_t st, LldLaunchInfo *info, bool launch)
 {
+  if (p.frameCenter != 0) return launch_g<M, F, NT, MINB, VEC2, true, F32, true>(p, numSMs, st, info, launch);
   if (p.opKind == 0 && p.magOut == nullptr) return launch_g<M, F, NT, MINB, VEC2, false, F32>(p, numSMs, st, info, launch);
   return launch_g<M, F, NT, MINB, VEC2, true, F32>(p, numSMs, st, info, launch);
 }

@@ -31,7 +31,7 @@ __global__ void __launch_bounds__(kLpcThreads) lpc_kernel(const LpcParams p)
   const long long uo = tp.uttOff[tl.utt];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int f = warp; f < tl.nf; f += kLpcWarps) {
-    FrameReader<F32> fr{tp, tp.pcm + (uo + (long long)(tl.f0 + f) * tp.frameStep) * tp.nChan};
+    FrameReader<F32> fr{tp, tp.pcm + uo * tp.nChan, frame_first_sample(tl.f0 + f, tp.frameStep, tp.frameCenter)};
     for (int n = lane; n < N; n += 32) xs[n] = tp.windowed ? fr.at(n) : fr.pre(n);
     __syncwarp();
     if (lane <= P) rs[f * (P + 1) + lane] = fm::acf_lag(xs, N, lane);

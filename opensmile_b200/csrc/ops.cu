@@ -396,7 +396,7 @@ __global__ void __launch_bounds__(32) energy_kernel(const TimeOpParams p)
   const int lane = threadIdx.x;
   if (lane >= tl.nf) return;
   const long long uo = p.uttOff[tl.utt];
-  FrameReader<F32> fr{p, p.pcm + (uo + (long long)(tl.f0 + lane) * p.frameStep) * p.nChan};
+  FrameReader<F32> fr{p, p.pcm + uo * p.nChan, frame_first_sample(tl.f0 + lane, p.frameStep, p.frameCenter)};
   const int N = p.frameSize;
   double d = 0.0;                                     // lldcore/energy.cpp:157-161
   for (int i = 0; i < N; i++) { const float t = fr.at(i); d += (double)__fmul_rn(t, t); }
@@ -424,7 +424,7 @@ __global__ void __launch_bounds__(32) mzcr_kernel(const TimeOpParams p)
   const int lane = threadIdx.x;
   if (lane >= tl.nf) return;
   const long long uo = p.uttOff[tl.utt];
-  FrameReader<F32> fr{p, p.pcm + (uo + (long long)(tl.f0 + lane) * p.frameStep) * p.nChan};
+  FrameReader<F32> fr{p, p.pcm + uo * p.nChan, frame_first_sample(tl.f0 + lane, p.frameStep, p.frameCenter)};
   const int N = p.frameSize;
   float mean = fr.at(0), nzc = 0.0f, nmc = 4.0f, mx = 0.f, mn = 0.f, absmax = 0.f;   // lldcore/mzcr.cpp:113-115
   if (p.zZcr || p.zMcr || p.zDc) {
@@ -471,7 +471,7 @@ __global__ void __launch_bounds__(32) intensity_kernel(const TimeOpParams p)
   const int lane = threadIdx.x;
   if (lane >= tl.nf) return;
   const long long uo = p.uttOff[tl.utt];
-  FrameReader<F32> fr{p, p.pcm + (uo + (long long)(tl.f0 + lane) * p.frameStep) * p.nChan};
+  FrameReader<F32> fr{p, p.pcm + uo * p.nChan, frame_first_sample(tl.f0 + lane, p.frameStep, p.frameCenter)};
   const int nOut = (p.iIntensity ? 1 : 0) + (p.iLoudness ? 1 : 0);
   const int safeN = min(p.frameSize, nOut);
   double Im = 0.0;

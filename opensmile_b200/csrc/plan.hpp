@@ -5,6 +5,7 @@
 #include <string>
 #include <vector>
 
+#include "frame_geom.cuh"
 #include "../../include/osm_b200.h"
 
 namespace osm {
@@ -63,8 +64,10 @@ struct FrontEnd {
   int format = OSM_B200_PCM_S16;
   bool mixdown = true;
   int frameSize = 0, frameStep = 0, nfft = 0, nBins = 0;
+  int frameCenter = 0;             // sampling centre in samples: frame t starts at t * frameStep - frameCenter (frame_geom.cuh)
   double frameSizeSec = 0;         // cFramer.frameSize (nominal)
   double frameStepSec = 0;
+  double timeOffset = 0;           // seconds added to the time of a frame's first sample (cFramer.frameCenter)
   double fftFrameSizeSec = 0;      // after cTransformFFT's rescale (transformFft.cpp:78-85)
   bool preemph = false;
   float preK = 0.f;

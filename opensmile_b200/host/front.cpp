@@ -314,7 +314,14 @@ bool to_component(const Section &s, osm_b200_component &c, std::string &err)
       case OSM_B200_C_FRAMER:
         SETD("frameSize", c.u.framer.frameSize) SETD("frameStep", c.u.framer.frameStep)
         SETI("noPostEOIprocessing", c.u.framer.noPostEOIprocessing)
-        if (f == "frameCenterSpecial") { c.u.framer.frameCenterSpecialLeft = (v.compare(0, 2, "le") == 0) ? 1 : 0; continue; }
+        SETD("frameCenter", c.u.framer.frameCenter)
+        if (f == "frameCenterFrames") { c.u.framer.frameCenterFrames = inum(v); c.u.framer.frameCenterFramesSet = 1; continue; }
+        if (f == "frameCenterSpecial") {   // core/winToVecProcessor.cpp:461-475: strncasecmp on the first two letters
+          std::string k = v.substr(0, 2);
+          for (char &ch : k) ch = (char)tolower((unsigned char)ch);
+          c.u.framer.frameCenterSpecial = (k == "mi" || k == "ce") ? OSM_B200_CENTER_MID : (k == "ri") ? OSM_B200_CENTER_RIGHT : OSM_B200_CENTER_LEFT;
+          continue;
+        }
         if (f == "frameMode") { if (v != "fixed") { err = "cFramer.frameMode=" + v + " is not supported"; return false; } continue; }
         if (f == "allowLastFrameIncomplete") { if (inum(v)) { err = "cFramer.allowLastFrameIncomplete=1 is not supported"; return false; } continue; }
         break;
