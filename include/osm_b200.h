@@ -47,7 +47,7 @@ extern "C" {
 /* 2: component types cSpecScale .. cPitchJitter appended (existing values and struct layouts unchanged)
  * 3: cSpecResample, cLpc, cFormantLpc, cDataSelector, cHarmonics appended (same rule; sizeof(osm_b200_component) grows);
  *    later cLsp appended under the same number: a new enum value at the end, no struct layout or size changes;
- *    cTonespec and cChroma likewise (their parameter blocks are smaller than the union); cTonefilt likewise */
+ *    cTonespec and cChroma likewise (their parameter blocks are smaller than the union); cTonefilt and cCens likewise */
 #define OSM_B200_ABI_VERSION 3
 #if defined(__GNUC__)
 #define OSM_B200_API __attribute__((visibility("default")))
@@ -104,6 +104,7 @@ typedef enum {
   OSM_B200_C_TONESPEC,           /* cTonespec           src/lld/tonespec.cpp:89-441 (on a cFFTmagphase magnitude level) */
   OSM_B200_C_CHROMA,             /* cChroma             src/lld/chroma.cpp:46-117 (on a cTonespec or cTonefilt level) */
   OSM_B200_C_TONEFILT,           /* cTonefilt           src/lld/tonefilt.cpp:65-259 (on the cWaveSource level) */
+  OSM_B200_C_CENS,               /* cCens               src/lld/cens.cpp:64-222 (on a cChroma level)      */
   OSM_B200_C_COUNT_
 } osm_b200_component_type;
 
@@ -379,6 +380,15 @@ typedef struct {            /* cTonefilt (lld/tonefilt.cpp:35-41) */
   double  outputPeriod;     /* 0.1 s */
 } osm_b200_tonefilt;
 
+typedef struct {            /* cCens (lld/cens.cpp:40-48) */
+  int32_t window;           /* OSM_B200_WIN_HANNING; HAMMING or BARTLETT (a window name the reference does not know is Hanning) */
+  int32_t winlength;        /* 41 taps; values < 1 become 1 */
+  int32_t l2norm;           /* 1 */
+  int32_t downsampleRatio;  /* 10; values < 1 become 1.  Scales the level's period only: every input row is an output row */
+  double  winlength_sec;    /* 0.41; used only when winlength_secSet (not supported: the reference crashes when it is set) */
+  int32_t winlength_secSet;
+} osm_b200_cens;
+
 /* one `[name:cType]` section */
 typedef struct {
   int32_t type;                                  /* osm_b200_component_type */
@@ -425,6 +435,7 @@ typedef struct {
     osm_b200_tonespec tonespec;
     osm_b200_chroma chroma;
     osm_b200_tonefilt tonefilt;
+    osm_b200_cens cens;
   } u;
 } osm_b200_component;
 
@@ -456,10 +467,13 @@ OSM_B200_API void            osm_b200_plan_destroy(osm_b200_plan *plan);
  * reference's naming rules (src/core/dataProcessor.cpp:249-325), e.g. "pcm_fftMag_mfcc[1]" */
 OSM_B200_API int32_t     osm_b200_plan_num_elements(const osm_b200_plan *plan);
 OSM_B200_API const char *osm_b200_plan_element_name(const osm_b200_plan *plan, int32_t idx);
-/* frame period of the output level in seconds (cFramer.frameStep) */
+/* period of the output level in seconds: cFramer.frameStep, cTonefilt.outputPeriod, and for a cCens level (and the levels behind
+ * it) its input's period times cCens.downsampleRatio (lld/cens.cpp:107-114).  It is the HTK sample period and the seconds unit of
+ * cFunctionals; it is not the spacing of a cCens level's row time stamps (osm_b200_plan_row_time). */
 OSM_B200_API double      osm_b200_plan_frame_period(const osm_b200_plan *plan);
-/* time stamp of row r of the output level: r * frame period for framer levels; (double)(r * P) / fs, the time of the row's first
- * sample, for a cTonefilt level (blocks of P samples; its period outputPeriod need not be P / fs) */
+/* time stamp of row r of the output level: r * cFramer.frameStep for framer levels; (double)(r * P) / fs, the time of the row's
+ * first sample, for a cTonefilt level (blocks of P samples; its period outputPeriod need not be P / fs).  A cCens level keeps the
+ * time stamps of its chroma rows (core/vectorProcessor.cpp:308): downsampleRatio scales the period only, not these times. */
 OSM_B200_API double      osm_b200_plan_row_time(const osm_b200_plan *plan, int64_t row);
 /* geometry resolved at plan time */
 OSM_B200_API int32_t     osm_b200_plan_frame_size_samples(const osm_b200_plan *plan);

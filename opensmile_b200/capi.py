@@ -22,7 +22,7 @@ OK, ERR_INVALID, ERR_UNSUPPORTED, ERR_CUDA, ERR_NOMEM = range(5)
  C_MELSPEC, C_MFCC, C_PLP, C_SPECTRAL, C_ENERGY, C_MZCR, C_ACF, C_PITCHACF,
  C_DELTAREGRESSION, C_CONTOURSMOOTHER, C_VECTORCONCAT, C_VECTOROPERATION, C_FULLINPUTMEAN, C_INTENSITY,
  C_SPECSCALE, C_PITCHSHS, C_PITCHSMOOTHERVITERBI, C_VALBASEDSELECTOR, C_PITCHJITTER,
- C_SPECRESAMPLE, C_LPC, C_FORMANTLPC, C_DATASELECTOR, C_HARMONICS, C_LSP, C_TONESPEC, C_CHROMA, C_TONEFILT) = range(34)
+ C_SPECRESAMPLE, C_LPC, C_FORMANTLPC, C_DATASELECTOR, C_HARMONICS, C_LSP, C_TONESPEC, C_CHROMA, C_TONEFILT, C_CENS) = range(35)
 
 # cTonespec.filterType (osm_b200_tone_filter)
 TONE_GAU, TONE_TRI, TONE_TRP, TONE_REC = range(4)
@@ -40,7 +40,7 @@ TYPE_BY_NAME = {
     "cValbasedSelector": C_VALBASEDSELECTOR, "cPitchJitter": C_PITCHJITTER,
     "cSpecResample": C_SPECRESAMPLE, "cLpc": C_LPC, "cFormantLpc": C_FORMANTLPC,
     "cDataSelector": C_DATASELECTOR, "cHarmonics": C_HARMONICS, "cLsp": C_LSP,
-    "cTonespec": C_TONESPEC, "cChroma": C_CHROMA, "cTonefilt": C_TONEFILT,
+    "cTonespec": C_TONESPEC, "cChroma": C_CHROMA, "cTonefilt": C_TONEFILT, "cCens": C_CENS,
 }
 
 WIN_BY_NAME = {"rec": 0, "han": 1, "ham": 2, "gau": 3, "sin": 4, "tri": 5, "bar": 6}
@@ -237,6 +237,11 @@ class Tonefilt(C.Structure):
     _fields_ = [("nNotes", i32), ("firstNote", f64), ("decayF0", f64), ("decayFN", f64), ("outputPeriod", f64)]
 
 
+class Cens(C.Structure):
+    _fields_ = [("window", i32), ("winlength", i32), ("l2norm", i32), ("downsampleRatio", i32), ("winlength_sec", f64),
+                ("winlength_secSet", i32)]
+
+
 class _U(C.Union):
     _fields_ = [("wavesource", WaveSource), ("framer", Framer),
                 ("vectorpreemphasis", VectorPreemphasis), ("windower", Windower),
@@ -249,7 +254,7 @@ class _U(C.Union):
                 ("valbasedselector", ValbasedSelector), ("pitchjitter", PitchJitter),
                 ("specresample", SpecResample), ("lpc", Lpc), ("formantlpc", FormantLpc),
                 ("dataselector", DataSelector), ("harmonics", Harmonics), ("lsp", Lsp),
-                ("tonespec", Tonespec), ("chroma", Chroma), ("tonefilt", Tonefilt)]
+                ("tonespec", Tonespec), ("chroma", Chroma), ("tonefilt", Tonefilt), ("cens", Cens)]
 
 
 class Component(C.Structure):
@@ -372,8 +377,8 @@ def lib():
         raise RuntimeError("ABI mismatch: sizeof(osm_b200_component) = %d, ctypes mirror = %d"
                            % (L.osm_b200_sizeof_component(), C.sizeof(Component)))
     L.osm_b200_tone_tables.argtypes = [C.POINTER(Tonespec), i32, f64, vp, vp, vp, vp, vp]
-    if L.osm_b200_component_defaults(C_TONEFILT, C.byref(Component())) != 0:     # the last component type of this mirror
-        raise RuntimeError("ABI mismatch: the library does not know component type %d (cTonefilt)" % C_TONEFILT)
+    if L.osm_b200_component_defaults(C_CENS, C.byref(Component())) != 0:     # the last component type of this mirror
+        raise RuntimeError("ABI mismatch: the library does not know component type %d (cCens)" % C_CENS)
     _lib = L
     return L
 

@@ -151,6 +151,11 @@ struct OpRt {
   PinBuf<ChunkRef> hSegs; DevBuf<ChunkRef> dSegs;
   std::vector<int32_t> uttSeg0; DevBuf<int32_t> dUttSeg0;
   DevBuf<double2> dAgg, dCin;
+  // cCens (SOP_CENS): its window, and tiles of the prepared batch (cut per utterance: rows do not depend on the batch)
+  CensParams cens;
+  DevBuf<float> dCensWin;
+  std::vector<int32_t> uttTile0;
+  PinBuf<OpTile> hCensTiles; DevBuf<OpTile> dCensTiles;
   int descOp = -1;                      // index into PlanDesc::ops
 };
 
@@ -318,6 +323,10 @@ osm_b200_status osm_b200_component_defaults(int32_t type, osm_b200_component *c)
     case OSM_B200_C_TONEFILT:              // lld/tonefilt.cpp:35-41
       c->u.tonefilt.nNotes = 48; c->u.tonefilt.firstNote = 55.0; c->u.tonefilt.decayF0 = 0.9995; c->u.tonefilt.decayFN = 0.998;
       c->u.tonefilt.outputPeriod = 0.1;
+      break;
+    case OSM_B200_C_CENS:                  // lld/cens.cpp:41-47
+      c->u.cens.window = OSM_B200_WIN_HANNING; c->u.cens.winlength = 41; c->u.cens.l2norm = 1; c->u.cens.downsampleRatio = 10;
+      c->u.cens.winlength_sec = 0.41; c->copyInputName = 0;
       break;
     case OSM_B200_C_HARMONICS: {           // lld/harmonics.cpp:28-56
       auto &q = c->u.harmonics;
@@ -924,7 +933,7 @@ try {
     OpRt rt;
     rt.kind = op.kind; rt.stream = op.stream; rt.descOp = (int)oi;
     StreamRt &srt = pl->st[op.stream];
-    if (op.kind != SOP_VECOP && op.kind != SOP_TONEFILT) srt.needTiles = true;      // the op reads its stream tile by tile
+    if (op.kind != SOP_VECOP && op.kind != SOP_TONEFILT && op.kind != SOP_CENS) srt.needTiles = true;      // the op reads its stream tile by tile
     if (op.kind == SOP_MAG) {
       rt.vN = d.streams[op.stream].fe.nBins; rt.vOutCol = op.outCol;
       rt.magMode = op.magMode; rt.magN = (float)d.streams[op.stream].fe.nfft; rt.magDbNorm = op.magDbNorm; rt.magMinDb = op.magMinDb;
@@ -932,6 +941,15 @@ try {
       const StaticOp &src = d.ops[op.srcOp];
       if (src.kind != SOP_MFCC && src.kind != SOP_PLP) return fail(OSM_B200_ERR_UNSUPPORTED, "cVectorOperation: the input must be a cMfcc / cPlp level");
       rt.vSrcCol = src.outCol; rt.vN = src.nOut; rt.vOutCol = op.outCol;
+    } else if (op.kind == SOP_CENS) {
+      const CensOp &co = op.cens;
+      if (cens_smem_bytes(co.N, co.W) > (size_t)prop.sharedMemPerBlockOptin) return fail(OSM_B200_ERR_UNSUPPORTED, "cCens: too many chroma elements for the kernel's shared memory");
+      CU(cens_configure(co.N, co.W, (size_t)prop.sharedMemPerBlockOptin));
+      CU(rt.dCensWin.upload(co.win.data(), co.win.size()));
+      CensParams &cp = rt.cens;
+      memset(&cp, 0, sizeof cp);
+      cp.srcCol = d.ops[op.srcOp].outCol; cp.outCol = op.outCol; cp.N = co.N; cp.W = co.W;
+      cp.win = rt.dCensWin.p; cp.l2norm = co.l2norm ? 1 : 0; cp.unit = co.unit;
     } else {
       const FrontEnd &fe = d.streams[op.stream].fe;
       switch (op.kind) {
@@ -979,7 +997,9 @@ const char *osm_b200_plan_element_name(const osm_b200_plan *pl, int32_t idx)
   return pl->d.names[idx].c_str();
 }
 
-double osm_b200_plan_frame_period(const osm_b200_plan *pl) { return pl ? pl->d.fe0().frameStepSec : 0.0; }
+// a cCens level's period is its input's times downsampleRatio; its rows keep the time stamps of their input rows (lld/cens.cpp:107-114,
+// core/vectorProcessor.cpp:308), so osm_b200_plan_row_time does not scale
+double osm_b200_plan_frame_period(const osm_b200_plan *pl) { return pl ? pl->d.fe0().frameStepSec * (double)pl->d.periodScale : 0.0; }
 double osm_b200_plan_row_time(const osm_b200_plan *pl, int64_t r)
 {
   if (!pl) return 0.0;
@@ -1131,6 +1151,22 @@ static osm_b200_status prepare_batch(osm_b200_plan *pl, const int64_t *uttOff, i
       CU(o.dCin.reserve(ns * o.tf.nNotes + 1));
       pl->totalWork += ns;
     }
+    for (OpRt &o : pl->ops) {
+      if (o.kind != SOP_CENS) continue;
+      std::vector<OpTile> tiles;
+      o.uttTile0.assign(nm, 0);
+      for (int u = 0; u < nUtt; u++) {
+        o.uttTile0[u] = (int32_t)tiles.size();
+        const int64_t Tu = desc_num_static_frames(d, o.stream, uttOff[u + 1] - uttOff[u]);
+        for (int64_t a = 0; a < Tu; a += kCensRows) tiles.push_back(OpTile{u, (int32_t)a, (int32_t)std::min<int64_t>(kCensRows, Tu - a), 0});
+      }
+      o.uttTile0[nUtt] = (int32_t)tiles.size();
+      CU(o.hCensTiles.reserve(tiles.size() + 1));
+      if (!tiles.empty()) memcpy(o.hCensTiles.p, tiles.data(), tiles.size() * sizeof(OpTile));
+      CU(o.dCensTiles.reserve(tiles.size() + 1));
+      if (!tiles.empty()) CU(cudaMemcpyAsync(o.dCensTiles.p, o.hCensTiles.p, tiles.size() * sizeof(OpTile), cudaMemcpyHostToDevice, st));
+      pl->totalWork += tiles.size();
+    }
     pl->totalRows = hR[nUtt];
     pl->totalStat = hS[nUtt];
     pl->totalSamples = uttOff[nUtt];
@@ -1248,7 +1284,7 @@ static osm_b200_status launch_range(osm_b200_plan *pl, const void *d_pcm, float 
       CU(cudaStreamWaitEvent(pl->auxStream, pl->evFork, 0));
       forked = true;
     }
-    if (o.kind == SOP_HARMONICS) continue;              // reads the pitch and formant columns: launched after the join below
+    if (o.kind == SOP_HARMONICS || o.kind == SOP_CENS) continue;   // read the columns of other ops: launched after the join below
     if (o.kind == SOP_TONEFILT) {
       const int s0 = o.uttSeg0[u0], s1 = o.uttSeg0[u1];
       if (s1 <= s0) continue;
@@ -1350,6 +1386,17 @@ static osm_b200_status launch_range(osm_b200_plan *pl, const void *d_pcm, float 
     CU(cudaStreamWaitEvent(st, pl->evJoin, 0));
   }
   for (OpRt &o : pl->ops) {
+    if (o.kind == SOP_CENS) {                           // the chroma columns (lld_kernel or tonefilt_kernel, both on `st`)
+      const int t0 = o.uttTile0[u0], t1 = o.uttTile0[u1];
+      if (t1 <= t0) continue;
+      CensParams cp = o.cens;
+      cp.stat = pl->dStat.p; cp.statStride = d.nStatic; cp.statOff = dS;
+      cp.tiles = o.dCensTiles.p + t0; cp.nTiles = t1 - t0;
+      CU(launch_cens(cp, st));
+      pl->lastLaunches++;
+      PROF("cens_kernel");
+      continue;
+    }
     if (o.kind != SOP_HARMONICS) continue;
     StreamRt &rt = pl->st[o.stream];
     const int t0 = rt.uttTile0[u0], t1 = rt.uttTile0[u1];

@@ -34,7 +34,7 @@ const char *type_name(int t)
     "cMZcr", "cAcf", "cPitchACF", "cDeltaRegression", "cContourSmoother", "cVectorConcat",
     "cVectorOperation", "cFullinputMean", "cIntensity", "cSpecScale", "cPitchShs", "cPitchSmootherViterbi",
     "cValbasedSelector", "cPitchJitter", "cSpecResample", "cLpc", "cFormantLpc", "cDataSelector", "cHarmonics", "cLsp",
-    "cTonespec", "cChroma", "cTonefilt"};
+    "cTonespec", "cChroma", "cTonefilt", "cCens"};
   return (t >= 0 && t < OSM_B200_C_COUNT_) ? names[t] : "?";
 }
 
@@ -51,6 +51,7 @@ const char *default_name_append(int t)
     case OSM_B200_C_TONESPEC: return "note";       // lld/tonespec.cpp:47
     case OSM_B200_C_CHROMA: return "chroma";       // lld/chroma.cpp:46
     case OSM_B200_C_TONEFILT: return "tonefilt";   // lld/tonefilt.cpp:35
+    case OSM_B200_C_CENS: return "CENS";           // lld/cens.cpp:41
     default: return "";
   }
 }
@@ -461,6 +462,7 @@ struct GraphCompiler {
       case OSM_B200_C_PITCHJITTER: s = build_jitter_op(c, op); break;
       case OSM_B200_C_TONESPEC: case OSM_B200_C_CHROMA: s = build_tone_op(c, op); break;
       case OSM_B200_C_TONEFILT: s = build_tonefilt_op(c, op); break;
+      case OSM_B200_C_CENS: s = build_cens_op(c, op); break;
       default: {
         char buf[512];
         snprintf(buf, sizeof buf, "component '%s' (%s) is not a supported static LLD producer", c->name, type_name(c->type));
@@ -468,7 +470,7 @@ struct GraphCompiler {
       }
     }
     if (s != OSM_B200_OK) return s;
-    if (op.kind != SOP_TONEFILT && op.kind != SOP_VECOP && d.streams[op.stream].fe.frameCenter != 0 && !centred_ok(op)) {
+    if (op.kind != SOP_TONEFILT && op.kind != SOP_VECOP && op.kind != SOP_CENS && d.streams[op.stream].fe.frameCenter != 0 && !centred_ok(op)) {
       char buf[512];
       snprintf(buf, sizeof buf, "component '%s' (%s) on a centred cFramer level (frameCenterSpecial / frameCenter / "
                "frameCenterFrames) is not supported", c->name, type_name(c->type));
@@ -721,6 +723,45 @@ struct GraphCompiler {
     if (!named.nameAppend[0]) snprintf(named.nameAppend, sizeof named.nameAppend, "%s", "lengthL1norm");
     const std::string inName = c->u.vectoroperation.nameBase[0] ? std::string(c->u.vectoroperation.nameBase) : d.ops[src].fields[0].name;
     add_field(op, name_append_auto(named, inName, nullptr));
+    return OSM_B200_OK;
+  }
+
+  // cCens on a cChroma level of either chroma front end (cTonespec or cTonefilt): a row-wise op on the chroma op's static columns
+  // (cens.cu).  Every input row gives an output row; downsampleRatio scales the level's period only (lld/cens.cpp:107-114,178).
+  osm_b200_status build_cens_op(const osm_b200_component *c, StaticOp &op)
+  {
+    const auto &q = c->u.cens;
+    if (c->n_inputs > 1) { err = std::string("cCens '") + c->name + "': a multi-field input (more than one input level) is not supported"; return OSM_B200_ERR_UNSUPPORTED; }
+    const osm_b200_component *in = single_input(c);
+    if (!in || in->type != OSM_B200_C_CHROMA) {
+      err = std::string("cCens '") + c->name + "' must read a cChroma level (it quantises chroma energies)"; return OSM_B200_ERR_UNSUPPORTED;
+    }
+    if (q.winlength_secSet) {
+      // lld/cens.cpp:91-100 reads the input level's period in myFetchConfig, before the reader's level is configured: the reference
+      // dereferences a null level configuration and crashes, so there is no behaviour to reproduce
+      err = std::string("cCens '") + c->name + "': winlength_sec is not supported (set winlength in frames)"; return OSM_B200_ERR_UNSUPPORTED;
+    }
+    const int W = q.winlength < 1 ? 1 : q.winlength;                    // :103
+    if (W > kCensMaxTaps) {
+      err = std::string("cCens '") + c->name + "': winlength " + std::to_string(W) + " is above " + std::to_string(kCensMaxTaps) + " taps";
+      return OSM_B200_ERR_UNSUPPORTED;
+    }
+    int src = -1;
+    osm_b200_status s2 = get_op(in, src);
+    if (s2 != OSM_B200_OK) return s2;
+    if (d.ops[src].fields.size() != 1) { err = std::string("cCens '") + c->name + "': the chroma level must hold exactly one field"; return OSM_B200_ERR_UNSUPPORTED; }
+    op.kind = SOP_CENS;
+    op.srcOp = src;
+    op.stream = d.ops[src].stream;
+    CensOp &co = op.cens;
+    co.N = d.ops[src].fields[0].n;
+    co.W = W;
+    co.l2norm = q.l2norm != 0;
+    co.ratio = q.downsampleRatio < 1 ? 1 : q.downsampleRatio;        // :102
+    const int win = q.window == OSM_B200_WIN_HAMMING || q.window == OSM_B200_WIN_BARTLETT ? q.window : OSM_B200_WIN_HANNING;
+    build_window(win, W, 0.0, 1.0, co.win);                             // (FLOAT_DMEM)_win[j], :123-128,185
+    co.unit = (float)(1.0 / std::sqrt((float)co.N));                    // :203, the float overload of sqrt
+    add_field(op, name_append_auto(*c, d.ops[src].fields[0].name, nullptr), co.N);
     return OSM_B200_OK;
   }
 
@@ -1158,6 +1199,13 @@ struct GraphCompiler {
     }
     if (stages.size() > 3) { err = "more than 3 chained temporal stages"; return OSM_B200_ERR_UNSUPPORTED; }
     const StaticOp &op = d.ops[opIdx];
+    // the level period: a cCens level's is its input's times downsampleRatio, and the levels behind it inherit it
+    const int ratio = op.kind == SOP_CENS ? op.cens.ratio : 1;
+    if (l > 0 && ratio != d.periodScale) {
+      err = "levels of different periods (a cCens level with downsampleRatio > 1 next to other levels) in one output level are not supported";
+      return OSM_B200_ERR_UNSUPPORTED;
+    }
+    d.periodScale = ratio;
     const size_t firstGroup = d.groups.size();
     int col = op.outCol;
     bool open = false;

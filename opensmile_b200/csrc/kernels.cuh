@@ -301,6 +301,23 @@ cudaError_t launch_tonefilt(const TonefiltParams &p, const int32_t *uttSeg0, int
 size_t tonefilt_smem_bytes(int nNotes, int chroma, size_t *sumsOffset);
 
 // ------------------------------------------------------------------------------------------
+// cCens on the N columns of a cChroma op (cens.cu): one CTA per tile of up to kCensRows rows of one utterance, the W - 1 rows in
+// front of the tile staged with it; the CENS rows overwrite columns outCol .. outCol + N - 1 of the static level
+// ------------------------------------------------------------------------------------------
+constexpr int kCensRows = 128;
+struct CensParams {
+  float *stat; int statStride; const long long *statOff;
+  const OpTile *tiles; int nTiles;   // rows [f0, f0 + nf) of utterance utt
+  int srcCol, outCol, N, W;
+  const float *win;                  // [W] (float)win[j]
+  int l2norm; float unit;            // unit: every element of a zero-norm row
+};
+cudaError_t launch_cens(const CensParams &p, cudaStream_t st);
+size_t cens_smem_bytes(int N, int W);
+// once per plan, on its device: the shared-memory limit the shape (N, W) needs (optinBytes = sharedMemPerBlockOptin)
+cudaError_t cens_configure(int N, int W, size_t optinBytes);
+
+// ------------------------------------------------------------------------------------------
 // SHS pitch chain (pitch.cu): cSpecScale + cPitchShs per frame (one warp per frame), cPitchSmootherViterbi
 // [+ cValbasedSelector] per utterance (one thread), cPitchJitter per utterance (one warp), and the temporal
 // stages of the levels behind them (one thread per utterance, seq_post_kernel).

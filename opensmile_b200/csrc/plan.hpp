@@ -58,6 +58,16 @@ struct TonefiltOp {
   float silThresh = 0.f;
 };
 
+// cCens (lld/cens.cpp:139-222) on the N columns of a cChroma op
+constexpr int kCensMaxTaps = 512;      // winlength bound of the kernel (cens.cu)
+struct CensOp {
+  int N = 12, W = 41;
+  bool l2norm = true;
+  int ratio = 1;                       // downsampleRatio: the level's period is the input's times ratio
+  std::vector<float> win;              // [W] (float)win[j]
+  float unit = 0.f;                    // (float)(1.0 / sqrt((float)N)): every element of a zero-norm row
+};
+
 struct FrontEnd {
   double sampleRate = 0;
   int nChan = 1;
@@ -80,7 +90,7 @@ struct FrontEnd {
   int rowSampleStep = 0;
 };
 
-enum StaticOpKind { SOP_MFCC = 0, SOP_PLP, SOP_MELSPEC, SOP_SPECTRAL, SOP_ENERGY, SOP_MZCR, SOP_PITCHACF, SOP_VECOP, SOP_MAG, SOP_INTENSITY, SOP_PITCH, SOP_JITTER, SOP_FORMANT, SOP_HARMONICS, SOP_LPC, SOP_TONE, SOP_TONEFILT };
+enum StaticOpKind { SOP_MFCC = 0, SOP_PLP, SOP_MELSPEC, SOP_SPECTRAL, SOP_ENERGY, SOP_MZCR, SOP_PITCHACF, SOP_VECOP, SOP_MAG, SOP_INTENSITY, SOP_PITCH, SOP_JITTER, SOP_FORMANT, SOP_HARMONICS, SOP_LPC, SOP_TONE, SOP_TONEFILT, SOP_CENS };
 
 struct MfccOp {
   int melIdx = 0;
@@ -239,7 +249,7 @@ struct StaticOp {
   bool windowed = false;           // time-domain ops: reads the windower level instead of the framer level
   int outCol = 0, nOut = 0;
   std::vector<FieldName> fields;   // names of the produced level
-  int srcOp = -1;                  // SOP_VECOP: op whose columns of the static level are reduced (ll1)
+  int srcOp = -1;                  // SOP_VECOP: op whose columns of the static level are reduced (ll1); SOP_CENS: the cChroma op
   int magMode = 0;                 // SOP_MAG: 0 magnitude, 1 normalise, 2 power, 3 both, 4 dBpsd (dspcore/fftmagphase.cpp:215-255)
   float magDbNorm = 0.f, magMinDb = 0.f;
   MfccOp mfcc;
@@ -256,6 +266,7 @@ struct StaticOp {
   LpcOp lpc;
   ToneOp tone;
   TonefiltOp tonefilt;
+  CensOp cens;
 };
 
 // temporal stage applied to a static column range (cWindowProcessor family)
@@ -303,6 +314,7 @@ struct PlanDesc {
   // The output level is the host layer's "_unionconcat" of the input levels of several cFunctionals instances: every level keeps
   // its own length (no min over the levels), the output has as many rows as the longest (rows past a level's end are not read)
   bool padRows = false;
+  int periodScale = 1;             // the output level's period = frameStepSec of stream 0 times this (cCens.downsampleRatio)
   const FrontEnd &fe0() const { return streams[0].fe; }
 };
 

@@ -239,7 +239,7 @@ const TypeInfo kTypes[] = {
   {"cPitchJitter", OSM_B200_C_PITCHJITTER}, {"cSpecResample", OSM_B200_C_SPECRESAMPLE}, {"cLpc", OSM_B200_C_LPC},
   {"cFormantLpc", OSM_B200_C_FORMANTLPC}, {"cDataSelector", OSM_B200_C_DATASELECTOR},
   {"cHarmonics", OSM_B200_C_HARMONICS}, {"cLsp", OSM_B200_C_LSP}, {"cTonespec", OSM_B200_C_TONESPEC}, {"cChroma", OSM_B200_C_CHROMA},
-  {"cTonefilt", OSM_B200_C_TONEFILT}};
+  {"cTonefilt", OSM_B200_C_TONEFILT}, {"cCens", OSM_B200_C_CENS}};
 
 // cTonespec.filterType spellings (lld/tonespec.cpp:107-111); any other value leaves the constructor's Gaussian (:83)
 int tone_filter(const std::string &f)
@@ -647,6 +647,17 @@ bool to_component(const Section &s, osm_b200_component &c, std::string &err)
         auto &q = c.u.tonefilt;
         SETI("nNotes", q.nNotes) SETD("firstNote", q.firstNote) SETD("decayF0", q.decayF0) SETD("decayFN", q.decayFN)
         SETD("outputPeriod", q.outputPeriod)
+        break;
+      }
+      case OSM_B200_C_CENS: {               // lld/cens.cpp:40-48, 64-105
+        auto &q = c.u.cens;
+        // strncmp on the first three characters, case-sensitive; any other string is Hanning (with an error message there)
+        if (f == "window") {
+          q.window = v.compare(0, 3, "ham") == 0 ? OSM_B200_WIN_HAMMING : (v.compare(0, 3, "bar") == 0 ? OSM_B200_WIN_BARTLETT : OSM_B200_WIN_HANNING);
+          continue;
+        }
+        SETI("winlength", q.winlength) SETI("l2norm", q.l2norm) SETI("downsampleRatio", q.downsampleRatio)
+        if (f == "winlength_sec") { q.winlength_sec = num(v); q.winlength_secSet = 1; continue; }
         break;
       }
       default: break;
