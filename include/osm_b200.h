@@ -507,6 +507,8 @@ OSM_B200_API int64_t     osm_b200_plan_num_frames_first_eoi_v(const osm_b200_pla
 /* per utterance of the last run: frames of the Viterbi level before the end-of-input flush (-1 when the plan has no SHS pitch chain);
  * synchronises the device */
 OSM_B200_API osm_b200_status osm_b200_plan_copy_seq_lag(osm_b200_plan *plan, int32_t *out, int32_t n_utt);
+/* the same values for a run enqueued on `stream` (cudaStream_t): waits for that stream only, never for the whole device */
+OSM_B200_API osm_b200_status osm_b200_plan_copy_seq_lag_stream(osm_b200_plan *plan, int32_t *out, int32_t n_utt, void *stream);
 
 /* number of distinct time stamps of those rows: frames of the level the first output field comes from, before its
  * window processors.  The rows a window processor appends at the end of input repeat the time stamp of the last
@@ -528,6 +530,17 @@ OSM_B200_API osm_b200_status osm_b200_plan_run_device(osm_b200_plan *plan, const
                                          const int64_t *frame_offsets, float *d_out,
                                          void *stream);
 
+/* Padded device batch, the layout a torch tensor [n_utt][n_channels][stride] has: channel-planar, utterance u's samples at
+ * d_pcm + u * n_channels * stride, lengths[u] <= stride sample frames (HOST array of n_utt entries; the padding is never read).
+ * Samples are int16 or float32 as the plan's cWaveSource.format says (OSM_B200_PCM_S16 / OSM_B200_PCM_F32; other formats are
+ * refused), its channel count is the plan's.  One kernel (pcm_pack_kernel) re-lays the batch out, without arithmetic, into a
+ * plan-owned buffer in the packed interleaved layout of osm_b200_plan_run_device, which then runs on it: rows are those of the
+ * same samples packed.  frame_offsets as returned by osm_b200_plan_frame_offsets for the offsets the lengths add up to (may be
+ * NULL).  Asynchronous on `stream`; like run_device, the plan's buffers are reused by its next run. */
+OSM_B200_API osm_b200_status osm_b200_plan_run_device_padded(osm_b200_plan *plan, const void *d_pcm, int64_t stride,
+                                                             const int64_t *lengths, int32_t n_utt,
+                                                             const int64_t *frame_offsets, float *d_out, void *stream);
+
 /* Host buffers: copies PCM to the device, runs, copies the rows back into `out`
  * (frame_offsets[n_utt] * num_elements floats) and synchronises. */
 OSM_B200_API osm_b200_status osm_b200_plan_run_host(osm_b200_plan *plan, const void *pcm,
@@ -548,6 +561,9 @@ OSM_B200_API int32_t     osm_b200_plan_last_launch_count(const osm_b200_plan *pl
  * kernel's workspace) and its row was zeroed.  osm_b200_plan_run_host checks this itself and fails with
  * OSM_B200_ERR_UNSUPPORTED; callers of the asynchronous osm_b200_plan_run_device ask here after their own sync. */
 OSM_B200_API int32_t     osm_b200_plan_take_device_flags(osm_b200_plan *plan);
+/* the same condition for a run enqueued on `stream`, as run_host reports it: OSM_B200_ERR_UNSUPPORTED (and the flag cleared)
+ * when it was raised.  Waits for `stream` only, and only when the plan has a cPitchJitter op: otherwise returns at once. */
+OSM_B200_API osm_b200_status osm_b200_plan_check_device_flags(osm_b200_plan *plan, void *stream);
 /* device time in ms of the fused LLD kernel(s) of the last run_* call, measured with CUDA
  * events on the run's stream; blocks until the run has finished.  <0 if unavailable. */
 OSM_B200_API float       osm_b200_plan_last_kernel_ms(osm_b200_plan *plan);

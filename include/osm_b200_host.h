@@ -86,6 +86,23 @@ OSM_B200_API osm_b200_status osm_b200_session_extract_pcm(osm_b200_session *sess
                                                           double sample_rate, int32_t n_channels,
                                                           int64_t *frame_offsets_out, float *out, int64_t max_rows);
 
+/* Extract from audio already in device memory: a padded batch [n_utt][n_channels][stride] (channel-planar, the layout of a
+ * contiguous torch tensor [B, C, L]; mono is n_channels = 1) of int16 (pcm_format = OSM_B200_PCM_S16) or float32
+ * (OSM_B200_PCM_F32) samples; lengths: HOST array of n_utt sample-frame counts <= stride (the padding is never read).  int16 samples
+ * are those of a 16-bit WAV file; float32 samples are taken as a 32-bit float WAV file holds them, without a full-scale division
+ * (e.g. values in [-1, 1]).  The rows are those osm_b200_session_extract_pcm / _extract_files give for the same samples.
+ * Same two-call protocol: d_out = NULL only fills frame_offsets_out (which needs a device exactly where extract_pcm's query does);
+ * otherwise d_out is a DEVICE buffer of at least max_rows * num_elements floats.  All work is enqueued on `stream` (cudaStream_t,
+ * NULL = default stream) and the call never synchronises the device: the host waits on `stream` only for the Viterbi lags of
+ * summary configurations with the SHS pitch chain, the cFunctionals row counts, and the cPitchJitter condition flag (reported as
+ * OSM_B200_ERR_UNSUPPORTED like extract_pcm).  An LLD configuration without cPitchJitter returns once its work is enqueued.
+ * The next call on the session, on any stream, starts after this call's work. */
+OSM_B200_API osm_b200_status osm_b200_session_extract_device(osm_b200_session *session, const void *d_pcm, int32_t pcm_format,
+                                                             int64_t stride, const int64_t *lengths, int32_t n_utt,
+                                                             double sample_rate, int32_t n_channels,
+                                                             int64_t *frame_offsets_out, float *d_out, int64_t max_rows,
+                                                             void *stream);
+
 /* the component list the session resolved (for diagnostics / tests): number of osm_b200_component
  * entries and a pointer to them (owned by the session, valid until close) */
 OSM_B200_API int32_t osm_b200_session_components(osm_b200_session *session, double sample_rate, int32_t n_channels,

@@ -287,6 +287,7 @@ EXPORTS = [
     "osm_b200_plan_frame_step_samples", "osm_b200_plan_fft_size", "osm_b200_plan_num_frames", "osm_b200_plan_num_time_frames",
     "osm_b200_plan_frame_offsets", "osm_b200_plan_run_device", "osm_b200_plan_run_host", "osm_b200_plan_run_host_resident",
     "osm_b200_window_table", "osm_b200_tone_tables", "osm_b200_plan_num_frames_first_eoi", "osm_b200_plan_num_frames_first_eoi_v", "osm_b200_plan_copy_seq_lag",
+    "osm_b200_plan_run_device_padded", "osm_b200_plan_copy_seq_lag_stream", "osm_b200_plan_check_device_flags",
     # include/osm_b200_functionals.h
     "osm_b200_functionals_defaults", "osm_b200_functionals_create", "osm_b200_functionals_destroy", "osm_b200_functionals_num_values",
     "osm_b200_functionals_num_elements", "osm_b200_functionals_element_name", "osm_b200_functionals_run_device", "osm_b200_functionals_run_device_cols", "osm_b200_summary_assemble_device", "osm_b200_plan_sample_frame_bytes", "osm_b200_device_csv_slot_bytes", "osm_b200_device_format_csv", "osm_b200_device_format_rows",
@@ -299,7 +300,7 @@ EXPORTS = [
     "osm_b200_session_open", "osm_b200_session_close", "osm_b200_session_num_elements",
     "osm_b200_session_element_name", "osm_b200_session_extract_files", "osm_b200_session_extract_files_arff", "osm_b200_session_sink_options",
     "osm_b200_session_write_files",
-    "osm_b200_session_extract_pcm", "osm_b200_session_components", "osm_b200_session_plan", "osm_b200_host_last_error",
+    "osm_b200_session_extract_pcm", "osm_b200_session_extract_device", "osm_b200_session_components", "osm_b200_session_plan", "osm_b200_host_last_error",
     "osm_b200_write_htk", "osm_b200_write_csv", "osm_b200_write_csv_timed", "osm_b200_write_arff",
 ]
 
@@ -348,6 +349,9 @@ def lib():
     L.osm_b200_plan_frame_offsets.argtypes = [vp, i64p, i32, i64p]
     L.osm_b200_plan_run_device.argtypes = [vp, vp, i64p, i32, i64p, vp, vp]
     L.osm_b200_plan_run_host.argtypes = [vp, vp, i64p, i32, i64p, vp]
+    L.osm_b200_plan_run_device_padded.argtypes = [vp, vp, C.c_int64, i64p, i32, i64p, vp, vp]
+    L.osm_b200_plan_copy_seq_lag_stream.argtypes = [vp, C.POINTER(i32), i32, vp]
+    L.osm_b200_plan_check_device_flags.argtypes = [vp, vp]
     L.osm_b200_plan_last_kernel_ms.argtypes = [vp]
     L.osm_b200_plan_last_kernel_ms.restype = C.c_float
     L.osm_b200_plan_last_kernel_times.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_float)]
@@ -369,6 +373,7 @@ def lib():
     L.osm_b200_session_write_files.argtypes = [vp, C.c_double, i32, i32, i64p, i64p, C.c_void_p, cpp, cpp, cpp]
     L.osm_b200_session_write_files.restype = i32
     L.osm_b200_session_extract_pcm.argtypes = [vp, vp, i64p, i32, f64, i32, i64p, vp, C.c_int64]
+    L.osm_b200_session_extract_device.argtypes = [vp, vp, i32, C.c_int64, i64p, i32, f64, i32, i64p, vp, C.c_int64, vp]
     L.osm_b200_session_components.argtypes = [vp, f64, i32, C.POINTER(C.POINTER(Component)), cpp]
     L.osm_b200_host_last_error.restype = C.c_char_p
     L.osm_b200_write_htk.argtypes = [C.c_char_p, vp, C.c_int64, i32, f64, i32]

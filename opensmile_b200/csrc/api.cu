@@ -91,6 +91,44 @@ __global__ void __launch_bounds__(256) pcm_convert_kernel(const unsigned char *i
   out[i] = __fdiv_rn(__fdiv_rn(tmp, (float)nChan), scale);
 }
 
+// A padded device batch -- [nUtt][nChan][stride] samples, channel-planar, the layout of a torch tensor -- re-laid out as the packed,
+// channel-interleaved batch the plan reads: the first uttOff[u + 1] - uttOff[u] sample frames of utterance u land at sample frame
+// uttOff[u].  Samples are moved as 2- or 4-byte words with no arithmetic, so the mixdown and conversion statements stay with the
+// kernels behind (pcm_convert_kernel, the int16 sample readers).  Samples past an utterance's length are never read.
+// Block (x, y): frames [x * tileF, (x + 1) * tileF) of utterances y, y + gridDim.y, ...  Mono is a straight copy; with several
+// channels the tile passes through shared memory ([nChan][tileF]) so that the planar reads and the interleaved writes both coalesce.
+constexpr int kPackThreads = 256;
+constexpr int kPackMonoFrames = 4096;           // frames per block of a mono batch
+constexpr int kPackTileBytes = 16 << 10;        // shared tile of a multi-channel batch
+template <typename T>
+__global__ void __launch_bounds__(kPackThreads) pcm_pack_kernel(const T *__restrict__ in, long long stride, int nChan, int tileF,
+                                                               const long long *__restrict__ uttOff, int nUtt, T *__restrict__ out)
+{
+  extern __shared__ __align__(16) unsigned char packSmem[];
+  T *tile = reinterpret_cast<T *>(packSmem);
+  const long long f0 = (long long)blockIdx.x * tileF;
+  for (int u = blockIdx.y; u < nUtt; u += gridDim.y) {
+    const long long o = uttOff[u], len = uttOff[u + 1] - o;
+    if (f0 >= len) continue;                                            // the same for every thread of the block
+    const int nf = (int)min((long long)tileF, len - f0);
+    const T *src = in + (size_t)u * nChan * stride + f0;
+    T *dst = out + (size_t)(o + f0) * nChan;
+    if (nChan == 1) {
+#pragma unroll 4
+      for (int t = threadIdx.x; t < nf; t += kPackThreads) dst[t] = src[t];
+      continue;
+    }
+    for (int c = 0; c < nChan; c++)
+      for (int t = threadIdx.x; t < nf; t += kPackThreads) tile[c * tileF + t] = src[(size_t)c * stride + t];
+    __syncthreads();
+    for (int k = threadIdx.x; k < nf * nChan; k += kPackThreads) {
+      const int t = k / nChan;
+      dst[k] = tile[(k - t * nChan) * tileF + t];
+    }
+    __syncthreads();                                                    // the tile is refilled for the next utterance
+  }
+}
+
 }  // namespace
 
 
@@ -192,6 +230,7 @@ struct osm_b200_plan {
   // run_host buffers
   DevBuf<int16_t> dPcm;
   DevBuf<float> dPcmF;             // mono float samples of the batch (inputs in another format than 16-bit integer)
+  DevBuf<unsigned char> dPadPcm;   // packed copy of a padded device batch (osm_b200_plan_run_device_padded)
   DevBuf<float> dOut;
   CudaStream hostStream, h2dStream, d2hStream;
   std::vector<CudaEvent> evPiece;   // 2 per pipeline piece: PCM landed / rows computed
@@ -1442,8 +1481,31 @@ static osm_b200_status launch_range(osm_b200_plan *pl, const void *d_pcm, float 
   return OSM_B200_OK;
 }
 
-osm_b200_status osm_b200_plan_run_device(osm_b200_plan *pl, const void *d_pcm, const int64_t *utt_offsets,
-                                         int32_t n_utt, const int64_t *frame_offsets, float *d_out, void *stream)
+// pcm_pack_kernel over the prepared batch: the padded batch d_pcm ([n_utt][nChan][stride]) into pl->dPadPcm
+static osm_b200_status launch_pack(osm_b200_plan *pl, const void *d_pcm, int64_t stride, int n_utt, int64_t maxLen, cudaStream_t st)
+{
+  const int nc = pl->d.fe0().nChan, sz = sample_bytes(pl->d.fe0().format);
+  CU(pl->dPadPcm.reserve((size_t)pl->totalSamples * nc * sz + 16));
+  if (maxLen == 0) return OSM_B200_OK;
+  const int tileF = nc == 1 ? kPackMonoFrames : std::max(1, std::min(kPackMonoFrames, kPackTileBytes / (nc * sz)));
+  const size_t smem = nc == 1 ? 0 : (size_t)tileF * nc * sz;
+  if (smem > 48 * 1024) return fail(OSM_B200_ERR_UNSUPPORTED, "padded device batch: too many channels for the packing kernel's tile");
+  const dim3 grid((unsigned)((maxLen + tileF - 1) / tileF), (unsigned)std::min(n_utt, 65535));
+  if (sz == 2)
+    pcm_pack_kernel<uint16_t><<<grid, kPackThreads, smem, st>>>(static_cast<const uint16_t *>(d_pcm), stride, nc, tileF, pl->dMeta.p, n_utt,
+                                                                reinterpret_cast<uint16_t *>(pl->dPadPcm.p));
+  else
+    pcm_pack_kernel<uint32_t><<<grid, kPackThreads, smem, st>>>(static_cast<const uint32_t *>(d_pcm), stride, nc, tileF, pl->dMeta.p, n_utt,
+                                                                reinterpret_cast<uint32_t *>(pl->dPadPcm.p));
+  CU(cudaGetLastError());
+  pl->lastLaunches++;
+  return OSM_B200_OK;
+}
+
+// run_device on a packed batch (padStride < 0), or on a padded one that is packed first (padStride = its stride, maxLen = the longest
+// utterance)
+static osm_b200_status run_device_impl(osm_b200_plan *pl, const void *d_pcm, const int64_t *utt_offsets, int32_t n_utt,
+                                       const int64_t *frame_offsets, float *d_out, void *stream, int64_t padStride, int64_t maxLen)
 {
   if (!pl || !utt_offsets || n_utt < 0) return fail(OSM_B200_ERR_INVALID, "null argument");
   if (pl->device < 0) return fail(OSM_B200_ERR_CUDA, "description-only plan (device < 0) cannot run; no CPU fallback");
@@ -1459,6 +1521,11 @@ osm_b200_status osm_b200_plan_run_device(osm_b200_plan *pl, const void *d_pcm, c
   if (!d_pcm || !d_out) return fail(OSM_B200_ERR_INVALID, "null device buffer");
   if (pl->d.fe0().format != OSM_B200_PCM_S16) CU(pl->dPcmF.reserve((size_t)utt_offsets[n_utt] + 16));
   if (!pl->staticDirect) CU(pl->dStat.reserve((size_t)pl->totalStat * pl->d.nStatic + 64));
+  if (padStride >= 0) {
+    s = launch_pack(pl, d_pcm, padStride, n_utt, maxLen, st);
+    if (s != OSM_B200_OK) return s;
+    d_pcm = pl->dPadPcm.p;
+  }
   CU(cudaEventRecord(pl->evK0, st));
   s = launch_range(pl, d_pcm, d_out, n_utt, 0, n_utt, st);
   if (s != OSM_B200_OK) return s;
@@ -1466,6 +1533,32 @@ osm_b200_status osm_b200_plan_run_device(osm_b200_plan *pl, const void *d_pcm, c
   pl->timed = true;
   return OSM_B200_OK;
 }
+
+osm_b200_status osm_b200_plan_run_device(osm_b200_plan *pl, const void *d_pcm, const int64_t *utt_offsets,
+                                         int32_t n_utt, const int64_t *frame_offsets, float *d_out, void *stream)
+{
+  return run_device_impl(pl, d_pcm, utt_offsets, n_utt, frame_offsets, d_out, stream, -1, 0);
+}
+
+// no exception crosses the C boundary (the utterance offsets are a host vector)
+osm_b200_status osm_b200_plan_run_device_padded(osm_b200_plan *pl, const void *d_pcm, int64_t stride, const int64_t *lengths,
+                                                int32_t n_utt, const int64_t *frame_offsets, float *d_out, void *stream)
+try {
+  if (!pl || !lengths || n_utt < 0) return fail(OSM_B200_ERR_INVALID, "null argument");
+  const int format = pl->d.fe0().format;
+  if (format != OSM_B200_PCM_S16 && format != OSM_B200_PCM_F32)
+    return fail(OSM_B200_ERR_INVALID, "a padded device batch holds int16 (OSM_B200_PCM_S16) or float32 (OSM_B200_PCM_F32) samples");
+  std::vector<int64_t> off((size_t)n_utt + 1, 0);
+  int64_t maxLen = 0;
+  for (int u = 0; u < n_utt; u++) {
+    if (lengths[u] < 0 || lengths[u] > stride)
+      return fail(OSM_B200_ERR_INVALID, "utterance " + std::to_string(u) + ": length " + std::to_string(lengths[u]) + " outside 0 .. stride (" +
+                                            std::to_string(stride) + ")");
+    off[u + 1] = off[u] + lengths[u];
+    maxLen = std::max(maxLen, lengths[u]);
+  }
+  return run_device_impl(pl, d_pcm, off.data(), n_utt, frame_offsets, d_out, stream, stride, maxLen);
+} catch (const std::bad_alloc &) { return fail(OSM_B200_ERR_NOMEM, "out of host memory"); }
 
 // Host buffers.  The batch is cut into pieces of whole utterances and pipelined over three
 // streams: H2D of piece k+1, kernels of piece k and D2H of piece k-1 overlap (the two copy
@@ -1542,13 +1635,23 @@ static osm_b200_status run_host_impl(osm_b200_plan *pl, const void *pcm, const i
   pl->timed = true;
   CU(cudaStreamSynchronize(pl->d2hStream));
   CU(cudaStreamSynchronize(st));
-  if (pl->dErr.p && pl->sp.nGroups + (int)pl->ops.size() > 0) {
-    int flag = 0;
-    CU(cudaMemcpy(&flag, pl->dErr.p, sizeof flag, cudaMemcpyDeviceToHost));
-    if (flag) {
-      CU(cudaMemset(pl->dErr.p, 0, sizeof(int)));
-      return fail(OSM_B200_ERR_UNSUPPORTED, "cPitchJitter: a frame left the supported geometry (F0 period / read window too long for the kernel's workspace); its rows were zeroed");
-    }
+  return osm_b200_plan_check_device_flags(pl, st);
+}
+
+osm_b200_status osm_b200_plan_check_device_flags(osm_b200_plan *pl, void *stream)
+{
+  if (!pl) return fail(OSM_B200_ERR_INVALID, "null plan");
+  // only cPitchJitter raises the flag: a plan without it has nothing to wait for
+  if (pl->device < 0 || std::none_of(pl->ops.begin(), pl->ops.end(), [](const OpRt &o) { return o.kind == SOP_JITTER; })) return OSM_B200_OK;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CU(cudaSetDevice(pl->device));
+  int flag = 0;
+  CU(cudaMemcpyAsync(&flag, pl->dErr.p, sizeof flag, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  if (flag) {
+    CU(cudaMemsetAsync(pl->dErr.p, 0, sizeof(int), st));
+    CU(cudaStreamSynchronize(st));
+    return fail(OSM_B200_ERR_UNSUPPORTED, "cPitchJitter: a frame left the supported geometry (F0 period / read window too long for the kernel's workspace); its rows were zeroed");
   }
   return OSM_B200_OK;
 }
@@ -1612,6 +1715,18 @@ osm_b200_status osm_b200_plan_copy_seq_lag(osm_b200_plan *pl, int32_t *out, int3
   CU(cudaDeviceSynchronize());
   if (!pl->ops[pl->seqLagOp].dLag.p) return OSM_B200_OK;
   CU(cudaMemcpy(out, pl->ops[pl->seqLagOp].dLag.p, sizeof(int) * (size_t)n_utt, cudaMemcpyDeviceToHost));
+  return OSM_B200_OK;
+}
+
+osm_b200_status osm_b200_plan_copy_seq_lag_stream(osm_b200_plan *pl, int32_t *out, int32_t n_utt, void *stream)
+{
+  if (!pl || !out || n_utt < 0) return fail(OSM_B200_ERR_INVALID, "null argument");
+  for (int u = 0; u < n_utt; u++) out[u] = -1;
+  if (pl->device < 0 || pl->seqLagOp < 0 || n_utt == 0 || !pl->ops[pl->seqLagOp].dLag.p) return OSM_B200_OK;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CU(cudaSetDevice(pl->device));
+  CU(cudaMemcpyAsync(out, pl->ops[pl->seqLagOp].dLag.p, sizeof(int) * (size_t)n_utt, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
   return OSM_B200_OK;
 }
 

@@ -1299,6 +1299,10 @@ struct osm_b200_session {
   std::map<std::pair<long, int>, FuncRt> funcs;
   FuncRt *curFunc = nullptr;
   osm::DevBuf<float> dFuncOut, dFuncScratch;
+  // osm_b200_session_extract_device: the LLD rows a summary configuration's plan leaves for its cFunctionals instances, and the
+  // end of the last call's work on its stream (the next call, on whatever stream, starts behind it: the buffers are reused)
+  osm::DevBuf<float> dLldRows;
+  osm::CudaEvent evDevice;
 
   // plans and functionals select their own device, the buffers above need it; a session without plans has made no CUDA call
   ~osm_b200_session() { if (device >= 0 && !plans.empty()) cudaSetDevice(device); }
@@ -1859,11 +1863,19 @@ osm_b200_status osm_b200_session_plan(osm_b200_session *s, double sampleRate, in
   return get_plan(s, sampleRate, nChan, plan);
 }
 
+// a padded device batch (osm_b200_session_extract_device): its samples, stride and lengths, and the stream its work goes to
+struct DeviceBatch { const void *pcm; int64_t stride; const int64_t *lengths; cudaStream_t stream; };
+
+// Both extract entry points: packed PCM in host memory with `out` in host memory (dev == NULL: the plan's pipelined host run, the
+// summary on the null stream, then a copy to `out`), or a padded device batch with `out` in device memory (every launch on
+// dev->stream; the host waits on that stream only where it needs device data or hands it host data: the Viterbi lags, the
+// cPitchJitter flag, the cFunctionals instances' row offsets and counts).
 static osm_b200_status osm_b200_session_extract_pcm_impl(osm_b200_session *s, const void *pcm, const int64_t *uttOff, int32_t nUtt,
                                              double sampleRate, int32_t nChan, int64_t *frameOff, float *out, int64_t maxRows,
-                                             int format = OSM_B200_PCM_S16)
+                                             int format = OSM_B200_PCM_S16, const DeviceBatch *dev = nullptr)
 {
   if (!s || !uttOff || !frameOff) return hfail(OSM_B200_ERR_INVALID, "null argument");
+  const cudaStream_t stream = dev ? dev->stream : nullptr;
   osm_b200_plan *p;
   osm_b200_status st = get_plan(s, sampleRate, nChan, &p, format);
   if (st != OSM_B200_OK) return st;
@@ -1901,14 +1913,22 @@ static osm_b200_status osm_b200_session_extract_pcm_impl(osm_b200_session *s, co
     auto now = [] { return std::chrono::steady_clock::now(); };
     auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
     const auto t0 = now();
-    st = osm_b200_plan_run_host_resident(p, pcm, uttOff, nUtt, lldOff.data(), &dRows);
+    if (dev) {
+      if (s->dLldRows.reserve((size_t)lldOff[(size_t)nUtt] * osm_b200_plan_num_elements(p)) != cudaSuccess)
+        return hfail(OSM_B200_ERR_NOMEM, "out of device memory (LLD rows)");
+      st = osm_b200_plan_run_device_padded(p, dev->pcm, dev->stride, dev->lengths, nUtt, lldOff.data(), s->dLldRows.p, stream);
+      if (st == OSM_B200_OK) st = osm_b200_plan_check_device_flags(p, stream);
+      dRows = s->dLldRows.p;
+    } else {
+      st = osm_b200_plan_run_host_resident(p, pcm, uttOff, nUtt, lldOff.data(), &dRows);
+    }
     if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
-    if (timing) cudaDeviceSynchronize();
+    if (timing) cudaStreamSynchronize(stream);
     const auto t1 = now();
     // levels behind the SHS pitch chain: their length at the first end-of-input tick follows the Viterbi level's (data dependent)
     {
       std::vector<int32_t> lag((size_t)nUtt, -1);
-      st = osm_b200_plan_copy_seq_lag(p, lag.data(), nUtt);
+      st = dev ? osm_b200_plan_copy_seq_lag_stream(p, lag.data(), nUtt, stream) : osm_b200_plan_copy_seq_lag(p, lag.data(), nUtt);
       if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
       for (size_t k = 0; k < live.size(); k++) {
         const int u = live[k];
@@ -1927,19 +1947,24 @@ static osm_b200_status osm_b200_session_extract_pcm_impl(osm_b200_session *s, co
       if (s->dFuncScratch.reserve_exact(needS) != cudaSuccess) return hfail(OSM_B200_ERR_NOMEM, "out of device memory (functionals scratch rows)");
       dInst = s->dFuncScratch.p;
     }
-    if (s->dFuncOut.reserve_exact(need) != cudaSuccess) return hfail(OSM_B200_ERR_NOMEM, "out of device memory (functionals rows)");
+    // the sink's rows: the caller's device buffer, or the session's, copied to the caller's host buffer below
+    float *dSink = out;
+    if (!dev) {
+      if (s->dFuncOut.reserve_exact(need) != cudaSuccess) return hfail(OSM_B200_ERR_NOMEM, "out of device memory (functionals rows)");
+      dSink = s->dFuncOut.p;
+    }
     for (size_t i = 0; i < nI; i++) {
       st = osm_b200_functionals_run_device_cols(f->f[i].get(), dRows, osm_b200_plan_num_elements(p), f->cols[i].data(), rowOff.data(), nRows[i].data(),
-                                                (int)live.size(), (dInst ? dInst : s->dFuncOut.p) + f->off[i], KS, nullptr);
+                                                (int)live.size(), (dInst ? dInst : dSink) + f->off[i], KS, stream);
       if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
     }
     if (dInst) {
-      st = osm_b200_summary_assemble_device(dInst, KS, f->gSrc.data(), f->gOp.data(), f->gFloor.data(), KF, (int64_t)live.size(), s->dFuncOut.p, KF, nullptr);
+      st = osm_b200_summary_assemble_device(dInst, KS, f->gSrc.data(), f->gOp.data(), f->gFloor.data(), KF, (int64_t)live.size(), dSink, KF, stream);
       if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
     }
-    if (timing) cudaDeviceSynchronize();
+    if (timing) cudaStreamSynchronize(stream);
     const auto t3 = now();
-    if (cudaMemcpy(out, s->dFuncOut.p, need * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess) return hfail(OSM_B200_ERR_CUDA, "copy of the functionals rows failed");
+    if (!dev && cudaMemcpy(out, s->dFuncOut.p, need * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess) return hfail(OSM_B200_ERR_CUDA, "copy of the functionals rows failed");
     if (timing) fprintf(stderr, "summary timing: LLD plan (H2D + kernels) %.2f ms, row counts %.2f ms, %zu cFunctionals instances + assemble %.2f ms, D2H %.2f ms\n",
                         ms(t0, t1), ms(t1, t2), nI, ms(t2, t3), ms(t3, now()));
     return OSM_B200_OK;
@@ -1948,8 +1973,22 @@ static osm_b200_status osm_b200_session_extract_pcm_impl(osm_b200_session *s, co
   if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
   if (!out) return OSM_B200_OK;
   if (frameOff[nUtt] > maxRows) return hfail(OSM_B200_ERR_INVALID, "output buffer too small");
-  st = osm_b200_plan_run_host(p, pcm, uttOff, nUtt, frameOff, out);
+  if (dev) {
+    st = osm_b200_plan_run_device_padded(p, dev->pcm, dev->stride, dev->lengths, nUtt, frameOff, out, stream);
+    if (st == OSM_B200_OK) st = osm_b200_plan_check_device_flags(p, stream);
+  } else {
+    st = osm_b200_plan_run_host(p, pcm, uttOff, nUtt, frameOff, out);
+  }
   if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
+  return OSM_B200_OK;
+}
+
+// The host-memory entry points reuse the plans and buffers whose last osm_b200_session_extract_device work may still be in flight on
+// its stream: they start after it.
+static osm_b200_status after_device_calls(osm_b200_session *s)
+{
+  if (s && s->evDevice && (cudaSetDevice(s->device) != cudaSuccess || cudaEventSynchronize(s->evDevice) != cudaSuccess))
+    return hfail(OSM_B200_ERR_CUDA, std::string("waiting for the last extract_device call: ") + cudaGetErrorString(cudaGetLastError()));
   return OSM_B200_OK;
 }
 
@@ -1957,10 +1996,40 @@ osm_b200_status osm_b200_session_extract_pcm(osm_b200_session *s, const int16_t 
                                              double sampleRate, int32_t nChan, int64_t *frameOff, float *out, int64_t maxRows)
 {
   // no exception crosses the C boundary (allocation failures on hostile inputs, std::filesystem / stream errors)
-  try { return osm_b200_session_extract_pcm_impl(s, pcm, uttOff, nUtt, sampleRate, nChan, frameOff, out, maxRows); }
+  try {
+    osm_b200_status st = after_device_calls(s);
+    return st != OSM_B200_OK ? st : osm_b200_session_extract_pcm_impl(s, pcm, uttOff, nUtt, sampleRate, nChan, frameOff, out, maxRows);
+  }
   catch (const std::bad_alloc &) { return hfail(OSM_B200_ERR_NOMEM, "out of host memory"); }
   catch (const std::exception &e) { return hfail(OSM_B200_ERR_INVALID, e.what()); }
 }
+
+osm_b200_status osm_b200_session_extract_device(osm_b200_session *s, const void *d_pcm, int32_t pcm_format, int64_t stride,
+                                                const int64_t *lengths, int32_t n_utt, double sample_rate, int32_t n_channels,
+                                                int64_t *frame_offsets_out, float *d_out, int64_t max_rows, void *stream)
+try {
+  if (!s || !lengths || !frame_offsets_out || n_utt < 0) return hfail(OSM_B200_ERR_INVALID, "null argument");
+  if (pcm_format != OSM_B200_PCM_S16 && pcm_format != OSM_B200_PCM_F32)
+    return hfail(OSM_B200_ERR_INVALID, "pcm_format must be OSM_B200_PCM_S16 (int16) or OSM_B200_PCM_F32 (float32)");
+  std::vector<int64_t> uttOff((size_t)n_utt + 1, 0);
+  for (int u = 0; u < n_utt; u++) {
+    if (lengths[u] < 0 || lengths[u] > stride)
+      return hfail(OSM_B200_ERR_INVALID, "utterance " + std::to_string(u) + ": length " + std::to_string(lengths[u]) + " outside 0 .. stride (" +
+                                             std::to_string(stride) + ")");
+    uttOff[(size_t)u + 1] = uttOff[(size_t)u] + lengths[u];
+  }
+  const DeviceBatch dev{d_pcm, stride, lengths, reinterpret_cast<cudaStream_t>(stream)};
+  // the row-count query touches no device; a run starts behind the previous call's work and marks the end of its own
+  const bool run = d_out && s->device >= 0;
+  if (run && (cudaSetDevice(s->device) != cudaSuccess || (s->evDevice && cudaStreamWaitEvent(dev.stream, s->evDevice, 0) != cudaSuccess)))
+    return hfail(OSM_B200_ERR_CUDA, std::string("extract_device: ") + cudaGetErrorString(cudaGetLastError()));
+  const osm_b200_status st = osm_b200_session_extract_pcm_impl(s, nullptr, uttOff.data(), n_utt, sample_rate, n_channels, frame_offsets_out,
+                                                               d_out, max_rows, pcm_format, &dev);
+  if (run && ((!s->evDevice && s->evDevice.create(cudaEventDisableTiming) != cudaSuccess) || cudaEventRecord(s->evDevice, dev.stream) != cudaSuccess))
+    return hfail(OSM_B200_ERR_CUDA, std::string("extract_device: ") + cudaGetErrorString(cudaGetLastError()));
+  return st;
+} catch (const std::bad_alloc &) { return hfail(OSM_B200_ERR_NOMEM, "out of host memory"); }
+catch (const std::exception &e) { return hfail(OSM_B200_ERR_INVALID, e.what()); }
 
 
 osm_b200_status osm_b200_session_extract_files(osm_b200_session *s, int32_t n, const char *const *wavPaths,
@@ -2037,6 +2106,7 @@ osm_b200_status osm_b200_session_extract_files_arff(osm_b200_session *s, int32_t
                                                     const char *const *arffPaths, int64_t *framesOut)
 try {
   if (!s || !wavPaths || n < 0) return hfail(OSM_B200_ERR_INVALID, "null argument");
+  if (osm_b200_status st = after_device_calls(s); st != OSM_B200_OK) return st;
   // files of one call are grouped by (sample rate, channels); each group is one batched plan run
   std::vector<Wav> wavs(n);
   std::string err;

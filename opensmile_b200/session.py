@@ -29,6 +29,7 @@ class Session:
     def __init__(self, conf_path, options=None, output_level=None, device=0):
         self._L = capi.lib()
         self._h = C.c_void_p()
+        self._device = device
         options = dict(options or {})
         st = self._L.osm_b200_session_open(
             str(conf_path).encode(), len(options), _strs(list(options.keys())), _strs(list(options.values())),
@@ -85,6 +86,58 @@ class Session:
             self._h, pcm.ctypes.data, off.ctypes.data_as(i64p), len(off) - 1, float(sample_rate), n_channels,
             fo.ctypes.data_as(i64p), out.ctypes.data, out.shape[0]))
         return out, fo
+
+    def extract_tensor(self, pcm, lengths, sample_rate):
+        """Audio already on the GPU -> (rows, frame_offsets), the pair extract_pcm returns, without a host round trip.
+
+        pcm: a contiguous CUDA tensor on the session's device, int16 or float32, shaped [B, L] (mono) or [B, C, L]
+        (channel-planar, as torch holds it); utterance b is its first lengths[b] samples, the padding is never read.
+        int16 samples are those of a 16-bit WAV file.  float32 samples are taken as a 32-bit float WAV file holds them,
+        e.g. torchaudio's values in [-1, 1]: they are not divided by a full scale (the reference's
+        smilePcm_convertFloatSamples).  Channels are mixed down as for a WAV file.
+        lengths: B sample-frame counts, a host sequence or a CPU tensor.
+        The work is enqueued on torch.cuda.current_stream(pcm.device).  rows: a CUDA float32 tensor
+        [frame_offsets[-1], num_elements] on pcm's device; frame_offsets: a numpy int64 array of B + 1 entries."""
+        import torch
+        if not isinstance(pcm, torch.Tensor):
+            raise TypeError("pcm must be a torch tensor")
+        fmt = {torch.int16: 0, torch.float32: 1}.get(pcm.dtype)       # OSM_B200_PCM_S16 / OSM_B200_PCM_F32
+        if fmt is None:
+            raise TypeError("pcm must be int16 or float32, not %s" % pcm.dtype)
+        if pcm.dim() not in (2, 3):
+            raise ValueError("pcm must be shaped [B, L] or [B, C, L], not %s" % (tuple(pcm.shape),))
+        if not pcm.is_contiguous():
+            raise ValueError("pcm must be contiguous (call .contiguous() on it: it is not copied here)")
+        n_utt, n_chan, stride = pcm.shape[0], (pcm.shape[1] if pcm.dim() == 3 else 1), pcm.shape[-1]
+        if isinstance(lengths, torch.Tensor):
+            if lengths.device.type != "cpu":
+                raise ValueError("lengths must be on the host (a sequence or a CPU tensor), not on %s" % lengths.device)
+            lengths = lengths.numpy()
+        lens = np.ascontiguousarray(lengths, dtype=np.int64)
+        if lens.shape != (n_utt,):
+            raise ValueError("lengths must hold %d entries (one per utterance), got shape %s" % (n_utt, lens.shape))
+        if n_utt and (lens.min() < 0 or lens.max() > stride):
+            raise ValueError("lengths must lie in 0 .. %d (the tensor's last dimension)" % stride)
+        if pcm.device.type != "cuda":
+            raise ValueError("pcm must be a CUDA tensor, not on %s" % pcm.device)
+        if pcm.device.index != self._device:
+            raise ValueError("pcm is on %s, the session runs on device %d" % (pcm.device, self._device))
+        i64p = C.POINTER(C.c_int64)
+        stream = C.c_void_p(torch.cuda.current_stream(pcm.device).cuda_stream)
+        fo = np.zeros(n_utt + 1, dtype=np.int64)
+
+        def call(d_out, max_rows):
+            self._check(self._L.osm_b200_session_extract_device(
+                self._h, C.c_void_p(pcm.data_ptr()), fmt, stride, lens.ctypes.data_as(i64p), n_utt, float(sample_rate), n_chan,
+                fo.ctypes.data_as(i64p), d_out, max_rows, stream))
+        call(None, 0)
+        n_el = self._L.osm_b200_session_num_elements(self._h, float(sample_rate), n_chan)
+        if n_el <= 0:
+            raise SessionError(capi.ERR_INVALID, self._L.osm_b200_host_last_error().decode())
+        rows = torch.empty((int(fo[-1]), n_el), dtype=torch.float32, device=pcm.device)
+        if rows.numel():
+            call(C.c_void_p(rows.data_ptr()), rows.shape[0])
+        return rows, fo
 
     def sink_options(self):
         """formatting options of the configuration's active sinks, as text (osm_b200_session_sink_options)"""
