@@ -16,8 +16,6 @@
 #include <sstream>
 #include <string>
 #include <vector>
-#include <functional>
-#include <chrono>
 #include <memory>
 
 #include "../../include/osm_b200_host.h"
@@ -56,6 +54,16 @@ std::string trim(const std::string &s)
   while (a < b && (s[a] == ' ' || s[a] == '\t' || s[a] == '\r' || s[a] == '\n')) a++;
   while (b > a && (s[b - 1] == ' ' || s[b - 1] == '\t' || s[b - 1] == '\r' || s[b - 1] == '\n')) b--;
   return s.substr(a, b - a);
+}
+
+// an `a;b;c` list (level lists, functionalsEnabled, array fields given in one line): items trimmed, empty items dropped
+std::vector<std::string> split_list(const std::string &v)
+{
+  std::vector<std::string> out;
+  std::stringstream ss(v);
+  std::string one;
+  while (std::getline(ss, one, ';')) { one = trim(one); if (!one.empty()) out.push_back(one); }
+  return out;
 }
 
 std::string dir_of(const std::string &p)
@@ -272,15 +280,10 @@ bool to_component(const Section &s, osm_b200_component &c, std::string &err)
   for (const auto &kv : s.kv) {
     const std::string &f = kv.first, &v = kv.second;
     if (f == "reader.dmLevel") {
-      std::stringstream ss(v);
-      std::string lv;
+      const std::vector<std::string> levels = split_list(v);
+      if (levels.size() > OSM_B200_MAX_INPUTS) { err = "too many input levels for '" + s.name + "'"; return false; }
       c.n_inputs = 0;
-      while (std::getline(ss, lv, ';')) {
-        lv = trim(lv);
-        if (lv.empty()) continue;
-        if (c.n_inputs >= OSM_B200_MAX_INPUTS) { err = "too many input levels for '" + s.name + "'"; return false; }
-        snprintf(c.reader_dmLevel[c.n_inputs++], OSM_B200_NAME_LEN, "%s", lv.c_str());
-      }
+      for (const std::string &l : levels) snprintf(c.reader_dmLevel[c.n_inputs++], OSM_B200_NAME_LEN, "%s", l.c_str());
       continue;
     }
     if (f == "writer.dmLevel") { snprintf(c.writer_dmLevel, sizeof c.writer_dmLevel, "%s", v.c_str()); continue; }
@@ -699,8 +702,9 @@ int time_norm(const std::string &v)          // functionalComponent.cpp:51-64: p
   return OSM_B200_TIMENORM_UNSET;
 }
 
-bool to_functionals(const Section &s, osm_b200_functionals_spec &fs, std::string &err)
+osm_b200_status to_functionals(const Section &s, osm_b200_functionals_spec &fs, std::string &err)
 {
+  auto fail = [&err](osm_b200_status st, const std::string &m) { err = m; return st; };
   osm_b200_functionals_defaults(&fs);
   std::map<int, std::string> enabledIdx;         // functionalsEnabled[i] entries
   std::string enabledList;
@@ -760,10 +764,10 @@ bool to_functionals(const Section &s, osm_b200_functionals_spec &fs, std::string
     const std::string &f = kv.first, &v = kv.second;
     // EOIlevel > 0 makes the summary wait for later end-of-input passes (more rows of the window processors behind it); a frame list
     // cuts the input into several summaries: both change what the rows mean and are refused rather than ignored
-    if (f == "EOIlevel" && inum(v) != 0) { err = "cFunctionals.EOIlevel != 0 is not supported (the summary is taken at the first end-of-input tick)"; return false; }
-    if ((f == "frameListFile" || f == "frameList") && !trim(v).empty()) { err = "cFunctionals." + f + " is not supported"; return false; }
+    if (f == "EOIlevel" && inum(v) != 0) return fail(OSM_B200_ERR_UNSUPPORTED, "cFunctionals.EOIlevel != 0 is not supported (the summary is taken at the first end-of-input tick)");
+    if ((f == "frameListFile" || f == "frameList") && !trim(v).empty()) return fail(OSM_B200_ERR_UNSUPPORTED, "cFunctionals." + f + " is not supported");
     if (is_common(f) || f == "noPostEOIprocessing" || f == "allowLastFrameIncomplete" || f == "frameListFile" || f == "frameList") continue;
-    if (f == "frameMode") { frameModeFull = true; if (v.compare(0, 3, "ful") != 0) { err = "cFunctionals.frameMode=" + v + " is not supported (only full-input summaries)"; return false; } continue; }
+    if (f == "frameMode") { frameModeFull = true; if (v.compare(0, 3, "ful") != 0) return fail(OSM_B200_ERR_UNSUPPORTED, "cFunctionals.frameMode=" + v + " is not supported (only full-input summaries)"); continue; }
     if (f == "frameSize" || f == "frameStep" || f == "frameSizeFrames" || f == "frameStepFrames") { if (num(v) != 0.0) subWindow = true; continue; }
     if (f == "frameCenterSpecial" || f == "frameCenter" || f == "frameCenterFrames") continue;
     if (f == "functionalsEnabled") { enabledList = v; continue; }
@@ -803,8 +807,8 @@ bool to_functionals(const Section &s, osm_b200_functionals_spec &fs, std::string
     }
     if (f.compare(0, 18, "Samples.samplepos[") == 0) { samplePos[atoi(f.c_str() + 18)] = num(v); continue; }
     if (f == "Samples.samplepos") {
-      std::stringstream ss(v); std::string one; int k = 0;
-      while (std::getline(ss, one, ';')) { one = trim(one); if (!one.empty()) samplePos[k++] = num(one); }
+      const std::vector<std::string> items = split_list(v);
+      for (size_t k = 0; k < items.size(); k++) samplePos[(int)k] = num(items[k]);
       continue;
     }
     if (f == "DCT.firstCoeff") { fs.dct.firstCoeff = std::max(0, inum(v)); continue; }          // functionalDCT.cpp:58-62
@@ -822,15 +826,14 @@ bool to_functionals(const Section &s, osm_b200_functionals_spec &fs, std::string
     if (f.compare(0, 22, "Percentiles.pctlrange[") == 0) { pctRange[atoi(f.c_str() + 22)] = v; continue; }
     // array fields given as one `a;b;c` list (core/configManager.cpp:2229-2262: the elements are assigned in order from index 0)
     if (f == "Percentiles.percentile" || f == "Percentiles.pctlrange") {
-      std::vector<std::string> items;
-      { std::stringstream ss(v); std::string one; while (std::getline(ss, one, ';')) { one = trim(one); if (!one.empty()) items.push_back(one); } }
+      const std::vector<std::string> items = split_list(v);
       for (size_t k = 0; k < items.size(); k++) { if (f == "Percentiles.percentile") pct[(int)k] = num(items[k]); else pctRange[(int)k] = items[k]; }
       continue;
     }
-    if (f.compare(0, 24, "Percentiles.pctlquotient") == 0 || f.compare(0, 15, "Percentiles.iqq") == 0) { err = "cFunctionalPercentiles: quotients are not supported"; return false; }
+    if (f.compare(0, 24, "Percentiles.pctlquotient") == 0 || f.compare(0, 15, "Percentiles.iqq") == 0) return fail(OSM_B200_ERR_UNSUPPORTED, "cFunctionalPercentiles: quotients are not supported");
     if (f.compare(0, 15, "Regression.qreg") == 0 && (f == "Regression.qregls" || f == "Regression.qregrs" || f == "Regression.qregx0" || f == "Regression.qregy0" ||
         f == "Regression.qregyr" || f == "Regression.qregy0nn" || f == "Regression.qregc3nn" || f == "Regression.qregyrnn")) {
-      if (inum(v)) { err = "cFunctionalRegression." + f.substr(11) + " is not supported"; return false; }
+      if (inum(v)) return fail(OSM_B200_ERR_UNSUPPORTED, "cFunctionalRegression." + f.substr(11) + " is not supported");
       continue;
     }
     bool hit = false;
@@ -845,12 +848,11 @@ bool to_functionals(const Section &s, osm_b200_functionals_spec &fs, std::string
       for (const char *k : known) other = other || sub == k;
       if (other) continue;
     }
-    err = "unknown field '" + f + "' in section [" + s.name + ":cFunctionals]";
-    return false;
+    return fail(OSM_B200_ERR_INVALID, "unknown field '" + f + "' in section [" + s.name + ":cFunctionals]");
   }
   fs.dct.lastCoeff = dctN >= 0 ? fs.dct.firstCoeff + dctN - 1 : dctLast;            // functionalDCT.cpp:63-68
   if (!samplePos.empty()) {                                                         // functionalSamples.cpp:50-66 (clipped to [0, 1])
-    if (samplePos.size() > OSM_B200_F_MAX_SAMPLES) { err = "cFunctionalSamples: more than 16 sample positions"; return false; }
+    if (samplePos.size() > OSM_B200_F_MAX_SAMPLES) return fail(OSM_B200_ERR_INVALID, "cFunctionalSamples: more than 16 sample positions");
     fs.samples.n_samplepos = 0;
     for (const auto &kv : samplePos) fs.samples.samplepos[fs.samples.n_samplepos++] = std::min(1.0, std::max(0.0, kv.second));
   }
@@ -860,17 +862,13 @@ bool to_functionals(const Section &s, osm_b200_functionals_spec &fs, std::string
   if (iqrSet) P.iqr12 = P.iqr23 = P.iqr13 = iqr;
   std::vector<std::string> names;
   if (!enabledIdx.empty()) for (const auto &kv : enabledIdx) names.push_back(trim(kv.second));
-  else {
-    std::stringstream ss(enabledList);
-    std::string one;
-    while (std::getline(ss, one, ';')) { one = trim(one); if (!one.empty()) names.push_back(one); }
-  }
-  if (names.empty()) { err = "cFunctionals '" + s.name + "': functionalsEnabled is empty"; return false; }
+  else names = split_list(enabledList);
+  if (names.empty()) return fail(OSM_B200_ERR_INVALID, "cFunctionals '" + s.name + "': functionalsEnabled is empty");
   // the reference's default frameMode is "fixed" (core/winToVecProcessor.cpp:66): a section that does not say frameMode = full
   // summarises sub-windows of frameSize seconds (MediaEval_Audio_IS12based_subwin2.conf: 2 s) -- not the full-input summary built here
-  if (!frameModeFull) { err = std::string("cFunctionals '") + s.name + "': frameMode = fixed (the default" + (subWindow ? ", with a frameSize" : "") + ") is not supported (only full-input summaries: frameMode = full)"; return false; }
+  if (!frameModeFull) return fail(OSM_B200_ERR_UNSUPPORTED, std::string("cFunctionals '") + s.name + "': frameMode = fixed (the default" + (subWindow ? ", with a frameSize" : "") + ") is not supported (only full-input summaries: frameMode = full)");
 
-  if (names.size() > OSM_B200_F_MAX_ENABLED) { err = "cFunctionals: too many enabled functionals"; return false; }
+  if (names.size() > OSM_B200_F_MAX_ENABLED) return fail(OSM_B200_ERR_INVALID, "cFunctionals: too many enabled functionals");
   fs.n_enabled = 0;
   for (const std::string &n : names) {
     int t = -1;
@@ -888,45 +886,41 @@ bool to_functionals(const Section &s, osm_b200_functionals_spec &fs, std::string
     else if (n == "Crossings") t = OSM_B200_F_CROSSINGS;
     else if (n == "Samples") t = OSM_B200_F_SAMPLES;
     else if (n == "DCT") t = OSM_B200_F_DCT;
-    else { err = "cFunctional" + n + " (instance '" + s.name + "') is not supported on the GPU path (Extremes, Means, Moments, Percentiles, Regression, Times, Lpc, Segments, Peaks2, Onset, Peaks, Crossings, Samples, DCT are)"; return false; }
-    if (t == OSM_B200_F_PEAKS && peaksNoOverlap) { err = "cFunctionalPeaks.overlapFlag = 0 (peak history carried from one contour to the next) is not supported"; return false; }
+    else return fail(OSM_B200_ERR_UNSUPPORTED, "cFunctional" + n + " (instance '" + s.name + "') is not supported on the GPU path (Extremes, Means, Moments, Percentiles, Regression, Times, Lpc, Segments, Peaks2, Onset, Peaks, Crossings, Samples, DCT are)");
+    if (t == OSM_B200_F_PEAKS && peaksNoOverlap) return fail(OSM_B200_ERR_UNSUPPORTED, "cFunctionalPeaks.overlapFlag = 0 (peak history carried from one contour to the next) is not supported");
     fs.enabled[fs.n_enabled++] = t;
-    if (t == OSM_B200_F_TIMES && unsupportedTimes) { err = "cFunctionalTimes: upleveltime[] / downleveltime[] arrays and useRobustPercentileRange are not supported"; return false; }
-    if (t == OSM_B200_F_PEAKS2 && unsupportedPeaks) { err = "cFunctionalPeaks2.noClearPeakList = 1 is not supported"; return false; }
+    if (t == OSM_B200_F_TIMES && unsupportedTimes) return fail(OSM_B200_ERR_UNSUPPORTED, "cFunctionalTimes: upleveltime[] / downleveltime[] arrays and useRobustPercentileRange are not supported");
+    if (t == OSM_B200_F_PEAKS2 && unsupportedPeaks) return fail(OSM_B200_ERR_UNSUPPORTED, "cFunctionalPeaks2.noClearPeakList = 1 is not supported");
     if (t == OSM_B200_F_SEGMENTS) {
-      if (unsupportedSeg) { err = "cFunctionalSegments: useOldBuggyChX / growDynSegBuffer are not supported"; return false; }
+      if (unsupportedSeg) return fail(OSM_B200_ERR_UNSUPPORTED, "cFunctionalSegments: useOldBuggyChX / growDynSegBuffer are not supported");
       // functionalSegments.cpp:124-158: prefix match in this order
       if (segAlgo.compare(0, 5, "relTh") == 0) SG.algorithm = OSM_B200_SEG_RELTH;
       else if (segAlgo.compare(0, 4, "nonX") == 0) SG.algorithm = OSM_B200_SEG_NONX;
       else if (segAlgo.compare(0, 3, "eqX") == 0) SG.algorithm = OSM_B200_SEG_EQX;
       else if (segAlgo.compare(0, 7, "NArelTh") == 0) SG.algorithm = OSM_B200_SEG_NARELTH;
-      else { err = "cFunctionalSegments.segmentationAlgorithm = " + segAlgo + " is not supported (relTh, NArelTh, nonX, eqX are)"; return false; }
+      else return fail(OSM_B200_ERR_UNSUPPORTED, "cFunctionalSegments.segmentationAlgorithm = " + segAlgo + " is not supported (relTh, NArelTh, nonX, eqX are)");
       std::vector<double> th;
       if (!segThresh.empty()) for (const auto &kv : segThresh) th.push_back(kv.second);
-      else {
-        std::stringstream ss(segThreshList);
-        std::string one;
-        while (std::getline(ss, one, ';')) { one = trim(one); if (!one.empty()) th.push_back(num(one)); }
-      }
+      else for (const std::string &one : split_list(segThreshList)) th.push_back(num(one));
       if (SG.algorithm == OSM_B200_SEG_RELTH && th.empty()) th.push_back(0.0);       // the field's default value
-      if (th.size() > OSM_B200_F_MAX_THRESH) { err = "cFunctionalSegments: more than 8 thresholds"; return false; }
+      if (th.size() > OSM_B200_F_MAX_THRESH) return fail(OSM_B200_ERR_INVALID, "cFunctionalSegments: more than 8 thresholds");
       SG.n_thresholds = (int)th.size();
       for (size_t k = 0; k < th.size(); k++) SG.thresholds[k] = (float)std::min(1.0, std::max(0.0, th[k]));   // :198-207
     }
   }
   P.n_percentile = 0;
   for (const auto &kv : pct) {
-    if (P.n_percentile >= OSM_B200_F_MAX_PCTL) { err = "cFunctionalPercentiles: more than 8 percentiles"; return false; }
+    if (P.n_percentile >= OSM_B200_F_MAX_PCTL) return fail(OSM_B200_ERR_INVALID, "cFunctionalPercentiles: more than 8 percentiles");
     P.percentile[P.n_percentile++] = std::min(1.0, std::max(0.0, kv.second));
   }
   P.n_pctlrange = 0;
   if (P.n_percentile > 0)
     for (const auto &kv : pctRange) {
       double a, b;
-      if (P.n_pctlrange >= OSM_B200_F_MAX_PCTL || !parse_range(kv.second, a, b)) { err = "cFunctionalPercentiles.pctlrange: expected X-Y"; return false; }
+      if (P.n_pctlrange >= OSM_B200_F_MAX_PCTL || !parse_range(kv.second, a, b)) return fail(OSM_B200_ERR_INVALID, "cFunctionalPercentiles.pctlrange: expected X-Y");
       P.pctlrange[P.n_pctlrange][0] = (int)a; P.pctlrange[P.n_pctlrange][1] = (int)b; P.n_pctlrange++;
     }
-  return true;
+  return OSM_B200_OK;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1233,7 +1227,8 @@ bool write_arff(const char *path, const float *rows, int64_t n, int K, const std
     }
     fputc('\n', f);
   }
-  fclose(f);
+  const bool bad = tb.failed || ferror(f) != 0;
+  if (fclose(f) != 0 || bad) { err = std::string("write error on '") + path + "'"; return false; }
   return true;
 }
 
@@ -1308,13 +1303,6 @@ struct osm_b200_session {
   ~osm_b200_session() { if (device >= 0 && !plans.empty()) cudaSetDevice(device); }
 };
 
-static void split_levels(const std::string &v, std::vector<std::string> &out)
-{
-  std::stringstream ss(v);
-  std::string one;
-  while (std::getline(ss, one, ';')) { one = trim(one); if (!one.empty()) out.push_back(one); }
-}
-
 static osm_b200_status get_plan(osm_b200_session *s, double sampleRate, int nChan, osm_b200_plan **out, int format = OSM_B200_PCM_S16)
 {
   const auto key = std::make_pair((long)lround(sampleRate * 1000.0), nChan + 4096 * format);
@@ -1360,6 +1348,44 @@ static osm_b200_status desc_plan(osm_b200_session *s, double sampleRate, int nCh
   const osm_b200_status st = osm_b200_plan_create(cs.data(), (int)cs.size(), lvl.c_str(), -1, &p);
   out.reset(p);
   return st == OSM_B200_OK ? OSM_B200_OK : hfail(st, osm_b200_last_error());
+}
+
+// one value of the sink's summary row: where it is in the scratch row, the operation applied to it, and its name
+struct SummEl { int src; int op; float fl; std::string name; };
+
+// the values summary node ni appends to `out`, over the instances' values in rt.f (their scratch row offsets rt.off)
+static bool eval_summary(const osm_b200_session *s, const osm_b200_session::FuncRt &rt, int ni, std::vector<SummEl> &out, std::string &err)
+{
+  const osm_b200_session::SummNode &nd = s->snodes[(size_t)ni];
+  if (nd.kind == 0) {
+    const int n = osm_b200_functionals_num_elements(rt.f[(size_t)nd.inst].get());
+    for (int j = 0; j < n; j++) out.push_back(SummEl{rt.off[(size_t)nd.inst] + j, OSM_B200_VOP_COPY, 0.f, osm_b200_functionals_element_name(rt.f[(size_t)nd.inst].get(), j)});
+    return true;
+  }
+  std::vector<SummEl> in;
+  for (int k : nd.kids) if (!eval_summary(s, rt, k, in, err)) return false;
+  if (nd.kind == 1) { out.insert(out.end(), in.begin(), in.end()); return true; }
+  if (nd.kind == 2) {                                               // core/dataSelector.cpp:296-366 (elementMode)
+    for (size_t k = 0; k < nd.sel.size(); k++) {
+      const SummEl *hit = nullptr;
+      for (const SummEl &e : in) if (e.name == nd.sel[k]) { hit = &e; break; }
+      if (!hit) { err = "cDataSelector: element '" + nd.sel[k] + "' not found in the summary levels it reads"; return false; }
+      SummEl e = *hit;
+      if (k < nd.newNames.size() && !nd.newNames[k].empty()) e.name = nd.newNames[k];
+      else if (!nd.nameAppend.empty()) e.name += "_" + nd.nameAppend;
+      out.push_back(e);
+    }
+    return true;
+  }
+  for (SummEl e : in) {                                             // other/vectorOperation.cpp:226-249 + core/dataProcessor.cpp:250-269
+    if (e.op != OSM_B200_VOP_COPY) { err = "chained cVectorOperation instances behind cFunctionals are not supported"; return false; }
+    const std::string base = !nd.nameBase.empty() ? nd.nameBase : e.name;
+    if (!nd.nameAppend.empty()) e.name = (nd.copyInputName && !base.empty()) ? base + "_" + nd.nameAppend : nd.nameAppend;
+    else e.name = (nd.copyInputName && !base.empty()) ? base : std::string("noname");
+    e.op = nd.op; e.fl = nd.logfloor;
+    out.push_back(e);
+  }
+  return true;
 }
 
 // the functionals objects of the session for one input format; device < 0: names / counts only
@@ -1422,42 +1448,9 @@ static osm_b200_status build_func_rt(osm_b200_session *s, double sampleRate, int
     rt.f.push_back(std::move(f)); rt.cols.push_back(cols); rt.desc.push_back(std::move(d));
   }
   // the sink's row: walk the summary graph over the instances' values
-  struct El { int src; int op; float fl; std::string name; };
-  std::string terr;
-  std::function<bool(int, std::vector<El> &)> eval = [&](int ni, std::vector<El> &out) -> bool {
-    const osm_b200_session::SummNode &nd = s->snodes[(size_t)ni];
-    if (nd.kind == 0) {
-      const int n = osm_b200_functionals_num_elements(rt.f[(size_t)nd.inst].get());
-      for (int j = 0; j < n; j++) out.push_back(El{rt.off[(size_t)nd.inst] + j, OSM_B200_VOP_COPY, 0.f, osm_b200_functionals_element_name(rt.f[(size_t)nd.inst].get(), j)});
-      return true;
-    }
-    std::vector<El> in;
-    for (int k : nd.kids) if (!eval(k, in)) return false;
-    if (nd.kind == 1) { out.insert(out.end(), in.begin(), in.end()); return true; }
-    if (nd.kind == 2) {                                               // core/dataSelector.cpp:296-366 (elementMode)
-      for (size_t k = 0; k < nd.sel.size(); k++) {
-        const El *hit = nullptr;
-        for (const El &e : in) if (e.name == nd.sel[k]) { hit = &e; break; }
-        if (!hit) { terr = "cDataSelector: element '" + nd.sel[k] + "' not found in the summary levels it reads"; return false; }
-        El e = *hit;
-        if (k < nd.newNames.size() && !nd.newNames[k].empty()) e.name = nd.newNames[k];
-        else if (!nd.nameAppend.empty()) e.name += "_" + nd.nameAppend;
-        out.push_back(e);
-      }
-      return true;
-    }
-    for (El e : in) {                                                 // other/vectorOperation.cpp:226-249 + core/dataProcessor.cpp:250-269
-      if (e.op != OSM_B200_VOP_COPY) { terr = "chained cVectorOperation instances behind cFunctionals are not supported"; return false; }
-      const std::string base = !nd.nameBase.empty() ? nd.nameBase : e.name;
-      if (!nd.nameAppend.empty()) e.name = (nd.copyInputName && !base.empty()) ? base + "_" + nd.nameAppend : nd.nameAppend;
-      else e.name = (nd.copyInputName && !base.empty()) ? base : std::string("noname");
-      e.op = nd.op; e.fl = nd.logfloor;
-      out.push_back(e);
-    }
-    return true;
-  };
-  std::vector<El> els;
-  if (!eval(s->sroot, els)) return hfail(OSM_B200_ERR_INVALID, terr);
+  std::vector<SummEl> els;
+  std::string err;
+  if (!eval_summary(s, rt, s->sroot, els, err)) return hfail(OSM_B200_ERR_INVALID, err);
   if (els.empty()) return hfail(OSM_B200_ERR_INVALID, "the summary level has no elements");
   rt.total = (int)els.size();
   rt.identity = rt.total == rt.scratch;
@@ -1484,6 +1477,354 @@ static osm_b200_status get_func(osm_b200_session *s, double sampleRate, int nCha
   return OSM_B200_OK;
 }
 
+// ------------------------------------------------------------------------------------------
+// osm_b200_session_open, pass by pass; the first error wins
+// ------------------------------------------------------------------------------------------
+// cCsvSink options (iocore/csvSink.cpp:40-54,78-110)
+static osm_b200_status read_csv_opts(const Section &sec, CsvOpts &o)
+{
+  o = CsvOpts();
+  if (const std::string *x = sec.get("printHeader")) o.printHeader = inum(*x) != 0;
+  if (const std::string *x = sec.get("timestamp")) o.timestamp = inum(*x) == 1;
+  if (const std::string *x = sec.get("frameTime")) o.timestamp = inum(*x) == 1;
+  if (const std::string *x = sec.get("number")) o.number = inum(*x) == 1;
+  if (const std::string *x = sec.get("frameIndex")) o.number = inum(*x) == 1;
+  if (const std::string *x = sec.get("instanceBase")) { o.instName = *x; o.prname = 2; }
+  if (const std::string *x = sec.get("instanceName")) { o.instName = *x; o.prname = 1; }
+  if (const std::string *x = sec.get("frameLength")) if (inum(*x) == 1) return hfail(OSM_B200_ERR_UNSUPPORTED, "cCsvSink.frameLength=1 is not supported");
+  if (const std::string *x = sec.get("delimChar")) if (!x->empty()) o.delim = *x == "<space>" ? ' ' : (*x == "<tab>" ? '\t' : (*x)[0]);
+  return OSM_B200_OK;
+}
+
+// cArffSink options (iocore/arffSink.cpp:40-170)
+static osm_b200_status read_arff_opts(const Section &sec, ArffOpts &a)
+{
+  a = ArffOpts();
+  if (const std::string *x = sec.get("relation")) a.relation = *x;
+  if (const std::string *x = sec.get("append")) a.append = inum(*x) != 0;
+  if (const std::string *x = sec.get("number")) a.number = inum(*x) == 1;
+  if (const std::string *x = sec.get("frameIndex")) a.number = inum(*x) == 1;
+  if (const std::string *x = sec.get("timestamp")) a.timestamp = inum(*x) == 1;
+  if (const std::string *x = sec.get("frameTime")) a.timestamp = inum(*x) == 1;
+  if (const std::string *x = sec.get("frameTimeAdd")) a.frameTimeAdd = num(*x);
+  if (const std::string *x = sec.get("printDefaultClassDummyAttribute")) a.dummyClass = inum(*x) != 0;
+  if (const std::string *x = sec.get("frameLength")) if (inum(*x) == 1) return hfail(OSM_B200_ERR_UNSUPPORTED, "cArffSink.frameLength=1 is not supported");
+  if (const std::string *x = sec.get("instanceBase")) if (!x->empty() && *x != "-") { a.instName = *x; a.prname = 2; }
+  if (const std::string *x = sec.get("instanceName")) if (!x->empty() && *x != "-") { a.instName = *x; a.prname = 1; }
+  for (int c = 0; c < 64; c++) {                       // class[c].name / class[c].type, target[c].all (:112-170)
+    char key[64];
+    snprintf(key, sizeof key, "class[%d].name", c);
+    const std::string *nm = sec.get(key);
+    snprintf(key, sizeof key, "class[%d].type", c);
+    const std::string *ty = sec.get(key);
+    if (!nm && !ty) break;
+    a.classes.push_back({nm ? *nm : std::string("class"), ty ? *ty : std::string("numeric")});
+    snprintf(key, sizeof key, "target[%d].all", c);
+    const std::string *tg = sec.get(key);
+    a.targetAll.push_back(tg ? (*tg == "?" ? *tg : arff_escape(*tg)) : std::string());
+    snprintf(key, sizeof key, "target[%d].instance[0]", c);
+    if (sec.get(key)) return hfail(OSM_B200_ERR_UNSUPPORTED, "cArffSink.target[].instance[] is not supported");
+  }
+  return OSM_B200_OK;
+}
+
+// pass 2: the instances listed in [componentInstances:cComponentManager] (core/componentManager.cpp:840-957) -> the compute
+// sections in order, the levels the active sinks read, and the sinks' options
+static osm_b200_status read_instances(osm_b200_session *s, std::vector<const Section *> &compute, std::vector<std::string> &sinkLevels)
+{
+  std::map<std::string, const Section *> secOf;
+  for (const auto &sec : s->conf.sections) if (sec.type != "cComponentManager") secOf[sec.name] = &sec;
+  bool csvLocked = false, arffLocked = false;
+  static const std::set<std::string> hostTypes = {"cDataMemory", "cHtkSink", "cCsvSink", "cArffSink", "cExternalSink", "cNullSink", "cDatadumpSink"};
+  for (const auto &inst : s->conf.instances) {
+    const std::string &name = inst.first, &type = inst.second;
+    const Section *sec = secOf.count(name) ? secOf[name] : nullptr;
+    if (sec && sec->type != type) return hfail(OSM_B200_ERR_INVALID, "instance '" + name + "' is declared as " + type + " but configured as " + sec->type);
+    if (hostTypes.count(type)) {
+      if (!sec || (type != "cHtkSink" && type != "cCsvSink" && type != "cArffSink" && type != "cExternalSink")) continue;
+      const std::string *fn = sec->get("filename");
+      const bool active = type == "cExternalSink" || (fn && *fn != "?" && !fn->empty());
+      const std::string *lv = sec->get("reader.dmLevel");
+      if (active && lv) sinkLevels.push_back(*lv);
+      if (type == "cArffSink" && active && !arffLocked) {
+        arffLocked = true;
+        if (osm_b200_status st = read_arff_opts(*sec, s->arff); st != OSM_B200_OK) return st;
+      }
+      if (type == "cHtkSink") { if (const std::string *pk = sec->get("parmKind")) s->parmKind = inum(*pk); }
+      // CSV formatting options: those of the active CSV sink; without one (explicit csv paths over the API),
+      // those of the last cCsvSink section
+      if (type == "cCsvSink" && !csvLocked) {
+        csvLocked = active;
+        if (osm_b200_status st = read_csv_opts(*sec, s->csv); st != OSM_B200_OK) return st;
+      }
+      continue;
+    }
+    if (!sec) return hfail(OSM_B200_ERR_INVALID, "instance '" + name + "' (" + type + ") has no configuration section");
+    compute.push_back(sec);
+  }
+  return OSM_B200_OK;
+}
+
+// pass 3: the output level: explicit, or the level the active sinks read; a multi-level sink reader is an
+// implicit concat (core/dataReader.cpp:360-444)
+static osm_b200_status choose_output_level(const char *output_level, const std::vector<std::string> &sinkLevels, std::string &lvl)
+{
+  lvl = output_level ? output_level : "";
+  if (!lvl.empty()) return OSM_B200_OK;
+  if (sinkLevels.empty()) return hfail(OSM_B200_ERR_INVALID, "no active sink: pass output_level or enable a sink (-O / -csvoutput)");
+  lvl = sinkLevels[0];
+  // every active sink gets the rows of ONE plan run: sinks that read different levels cannot be served together
+  for (const std::string &l : sinkLevels)
+    if (l != lvl) return hfail(OSM_B200_ERR_UNSUPPORTED, "the active sinks read different levels ('" + lvl + "' and '" + l + "'): enable the sinks of one level per session");
+  return OSM_B200_OK;
+}
+
+// a cDataSelector section (core/dataSelector.cpp:296-366, elementMode): the element names it selects, the new names it gives
+// them, the text it appends to their names, and the first field the summary path does not model ("" if there is none)
+struct Selector { std::vector<std::string> sel, newNames; std::string nameAppend, unsupported; bool renames = false; };
+
+static Selector read_selector(const Section &ds)
+{
+  Selector r;
+  std::map<int, std::string> selIdx, newIdx;
+  std::string selList, newList;
+  for (const auto &kv : ds.kv) {
+    const std::string &f = kv.first;
+    if (f == "nameAppend") { r.nameAppend = kv.second; continue; }
+    if (is_common(f) || f == "reader.dmLevel" || f == "writer.dmLevel") continue;
+    if (f == "selected") selList = kv.second;
+    else if (f.compare(0, 9, "selected[") == 0) selIdx[atoi(f.c_str() + 9)] = kv.second;
+    else if (f == "newNames") { newList = kv.second; r.renames = true; }
+    else if (f.compare(0, 9, "newNames[") == 0) { newIdx[atoi(f.c_str() + 9)] = kv.second; r.renames = true; }
+    else if (r.unsupported.empty() && (f != "elementMode" || inum(kv.second) != 1)) r.unsupported = f;
+  }
+  if (!selIdx.empty()) for (const auto &kv : selIdx) r.sel.push_back(trim(kv.second));
+  else r.sel = split_list(selList);
+  if (!newIdx.empty()) {
+    r.newNames.assign(r.sel.size(), "");
+    for (const auto &kv : newIdx) if (kv.first >= 0 && (size_t)kv.first < r.newNames.size()) r.newNames[(size_t)kv.first] = trim(kv.second);
+  } else r.newNames = split_list(newList);
+  return r;
+}
+
+static bool summary_glue(const std::string &type) { return type == "cVectorConcat" || type == "cDataSelector" || type == "cVectorOperation"; }
+
+// pass 4: the summary graph behind the output level -- cFunctionals levels below cVectorConcat (any depth), cDataSelector and
+// cVectorOperation nodes.  Fills the session's finsts, snodes, sroot and unionLevels (the instances' reader levels, which the
+// plan computes; the summaries then run on the resident rows, functionals.cu, each instance on its columns).
+struct SummaryBuilder {
+  osm_b200_session &s;
+  const std::map<std::string, const Section *> &writerOf;      // level -> the compute section that writes it
+  std::map<const Section *, int> instOf;                       // cFunctionals section -> its index in s.finsts
+  osm_b200_status status = OSM_B200_OK;
+  std::string msg;
+
+  int fail(osm_b200_status st, const std::string &m) { status = st; msg = m; return -1; }
+
+  bool has_functionals(const std::string &level, int depth) const
+  {
+    auto it = writerOf.find(level);
+    if (it == writerOf.end() || depth > 16) return false;
+    const Section &w = *it->second;
+    if (w.type == "cFunctionals") return true;
+    const std::string *r = w.get("reader.dmLevel");
+    if (!summary_glue(w.type) || !r) return false;
+    for (const std::string &l : split_list(*r)) if (has_functionals(l, depth + 1)) return true;
+    return false;
+  }
+
+  // the instance of cFunctionals section w, added on first use; -1 on error
+  int add_instance(const Section &w)
+  {
+    auto it = instOf.find(&w);
+    if (it != instOf.end()) return it->second;
+    osm_b200_session::FuncInst fi;
+    std::string err;
+    if (osm_b200_status st = to_functionals(w, fi.spec, err); st != OSM_B200_OK) return fail(st, err);
+    if (const std::string *x = w.get("preserveFields")) fi.preserveFields = inum(*x) != 0;
+    const std::string *r = w.get("reader.dmLevel");
+    if (!r) return fail(OSM_B200_ERR_INVALID, "cFunctionals '" + w.name + "' has no reader.dmLevel");
+    for (const std::string &l : split_list(*r)) {
+      osm_b200_session::FuncReader rd;
+      rd.level = l;
+      // a cDataSelector that only picks named elements (and appends to their names) is a view of its input level
+      auto itw = writerOf.find(l);
+      if (itw != writerOf.end() && itw->second->type == "cDataSelector") {
+        Selector sel = read_selector(*itw->second);
+        const std::string *base = itw->second->get("reader.dmLevel");
+        if (sel.unsupported.empty() && !sel.renames && base && base->find(';') == std::string::npos && !sel.sel.empty()) {
+          rd.level = trim(*base);
+          rd.sel = std::move(sel.sel);
+          rd.nameAppend = sel.nameAppend;
+        }
+      }
+      fi.readers.push_back(rd);
+      if (std::find(s.unionLevels.begin(), s.unionLevels.end(), rd.level) == s.unionLevels.end()) s.unionLevels.push_back(rd.level);
+    }
+    s.finsts.push_back(fi);
+    return instOf[&w] = (int)s.finsts.size() - 1;
+  }
+
+  // the node of s.snodes that produces `level`; -1 on error
+  int build_node(const std::string &level, int depth)
+  {
+    auto it = writerOf.find(level);
+    if (it == writerOf.end() || depth > 16) return fail(OSM_B200_ERR_INVALID, "level '" + level + "' has no writer");
+    const Section &w = *it->second;
+    osm_b200_session::SummNode nd;
+    if (w.type == "cFunctionals") {
+      nd.kind = 0;
+      nd.inst = add_instance(w);
+      if (nd.inst < 0) return -1;
+      s.snodes.push_back(nd);
+      return (int)s.snodes.size() - 1;
+    }
+    const std::string *r = w.get("reader.dmLevel");
+    if (!r || !summary_glue(w.type))
+      return fail(OSM_B200_ERR_UNSUPPORTED, "a level that mixes cFunctionals summaries with other levels is not supported (level '" + level + "')");
+    const std::vector<std::string> rl = split_list(*r);
+    for (const std::string &l : rl) { const int k = build_node(l, depth + 1); if (k < 0) return -1; nd.kids.push_back(k); }
+    if (w.type == "cVectorConcat") {
+      // summary levels hold single-element fields: a cVectorConcat that keeps only array fields (its default) would be empty
+      nd.kind = 1;
+      int paf = 1, incl = 0;
+      if (const std::string *x = w.get("processArrayFields")) paf = inum(*x);
+      if (const std::string *x = w.get("includeSingleElementFields")) incl = inum(*x);
+      if (paf == 1 && !incl && rl.size() > 1)
+        return fail(OSM_B200_ERR_UNSUPPORTED, "cVectorConcat '" + w.name + "' behind cFunctionals drops single-element fields (includeSingleElementFields = 0)");
+    } else if (w.type == "cDataSelector") {
+      nd.kind = 2;
+      Selector sel = read_selector(w);
+      if (sel.unsupported == "elementMode") return fail(OSM_B200_ERR_UNSUPPORTED, "cDataSelector.elementMode=0 is not supported");
+      if (!sel.unsupported.empty()) return fail(OSM_B200_ERR_UNSUPPORTED, "cDataSelector '" + w.name + "': field '" + sel.unsupported + "' is not supported");
+      if (sel.sel.empty()) return fail(OSM_B200_ERR_INVALID, "cDataSelector '" + w.name + "': no elements selected");
+      nd.sel = std::move(sel.sel);
+      nd.newNames = std::move(sel.newNames);
+      nd.nameAppend = sel.nameAppend;
+    } else {
+      nd.kind = 3;                                                  // other/vectorOperation.cpp:42-48,136-139,210-222
+      std::string opn = "norm";
+      int appendOp = 0;
+      double lf = 1e-12;                                            // default of `logfloor`
+      for (const auto &kv : w.kv) {
+        const std::string &f = kv.first;
+        if (f == "nameAppend") { nd.nameAppend = kv.second; continue; }
+        if (f == "copyInputName") { nd.copyInputName = inum(kv.second) != 0; continue; }
+        if (is_common(f) || f == "reader.dmLevel" || f == "writer.dmLevel") continue;
+        if (f == "operation") opn = kv.second;
+        else if (f == "nameBase") nd.nameBase = kv.second;
+        else if (f == "appendOperationToName") appendOp = inum(kv.second);
+        else if (f == "logfloor") lf = atof(kv.second.c_str());
+        else if (f == "processArrayFields" || f == "includeSingleElementFields" || f == "param1" || f == "param2" || f == "powOnlyPos") continue;
+        else return fail(OSM_B200_ERR_UNSUPPORTED, "cVectorOperation '" + w.name + "': field '" + f + "' is not supported");
+      }
+      if (opn.compare(0, 3, "dBp") == 0) nd.op = OSM_B200_VOP_DBP;
+      else if (opn.compare(0, 3, "dBv") == 0) nd.op = OSM_B200_VOP_DBV;
+      else return fail(OSM_B200_ERR_UNSUPPORTED, "cVectorOperation behind cFunctionals: only operation = dBp / dBv is supported (got '" + opn + "')");
+      if (appendOp) nd.nameAppend = opn;                             // overrides nameAppend (:210-216, :240-243)
+      if (lf <= 0) lf = 0.000000000001;                              // :219-223
+      nd.logfloor = (float)lf;
+      if (rl.size() != 1) return fail(OSM_B200_ERR_UNSUPPORTED, "cVectorOperation must read exactly one level");
+    }
+    s.snodes.push_back(nd);
+    return (int)s.snodes.size() - 1;
+  }
+};
+
+// pass 4 on the output level: with cFunctionals behind it, the output level becomes the union of the instances' reader levels
+static osm_b200_status build_summary(osm_b200_session *s, const std::map<std::string, const Section *> &writerOf)
+{
+  SummaryBuilder b{*s, writerOf};
+  const std::vector<std::string> parts = split_list(s->outputLevel);
+  bool anyFunc = false;
+  for (const std::string &pl : parts) anyFunc = anyFunc || b.has_functionals(pl, 0);
+  if (!anyFunc) return OSM_B200_OK;
+  osm_b200_session::SummNode root;
+  root.kind = 1;
+  for (const std::string &pl : parts) {
+    const int k = b.build_node(pl, 0);
+    if (k < 0) return hfail(b.status, b.msg);
+    root.kids.push_back(k);
+  }
+  if (parts.size() == 1) s->sroot = root.kids[0];
+  else { s->snodes.push_back(root); s->sroot = (int)s->snodes.size() - 1; }
+  if (s->unionLevels.size() > OSM_B200_MAX_INPUTS) return hfail(OSM_B200_ERR_UNSUPPORTED, "cFunctionals: more than 8 input levels in total");
+  s->hasFunc = true;
+  s->outputLevel.clear();
+  for (const std::string &l : s->unionLevels) s->outputLevel += (s->outputLevel.empty() ? "" : ";") + l;
+  return OSM_B200_OK;
+}
+
+// pass 5: only the components the output level depends on are part of the plan: the shipped feature-set
+// configurations carry sinks and summaries (cFunctionals ...) that stay idle when their output file is
+// not requested (filename = ?), exactly like the reference leaves those sinks unwritten.
+static osm_b200_status lower_sections(osm_b200_session *s, const std::vector<const Section *> &compute,
+                                      const std::map<std::string, const Section *> &writerOf)
+{
+  std::set<const Section *> need;
+  std::vector<std::string> todo = split_list(s->outputLevel);
+  while (!todo.empty()) {
+    const std::string l = todo.back();
+    todo.pop_back();
+    auto it = writerOf.find(l);
+    if (it == writerOf.end() || need.count(it->second)) continue;
+    need.insert(it->second);
+    for (const char *key : {"reader.dmLevel", "reader2.dmLevel", "F0reader.dmLevel"})
+      if (const std::string *r = it->second->get(key))
+        for (const std::string &more : split_list(*r)) todo.push_back(more);
+  }
+  for (const Section *sec : compute) {
+    const bool isWave = sec->type == "cWaveSource" || sec->type == "cExternalAudioSource";
+    if (!isWave && !need.count(sec)) continue;
+    osm_b200_component c;
+    std::string err;
+    if (!to_component(*sec, c, err)) return hfail(type_of(sec->type) < 0 ? OSM_B200_ERR_UNSUPPORTED : OSM_B200_ERR_INVALID, err);
+    if (c.type == OSM_B200_C_WAVESOURCE) s->waveIdx = (int)s->comps.size();
+    s->comps.push_back(c);
+  }
+  if (s->waveIdx < 0) return hfail(OSM_B200_ERR_INVALID, "the configuration has no cWaveSource / cExternalAudioSource");
+  return OSM_B200_OK;
+}
+
+// pass 6: an output level of several levels is read through one concat component
+static osm_b200_status add_reader_concat(osm_b200_session *s)
+{
+  if (s->outputLevel.find(';') == std::string::npos) return OSM_B200_OK;
+  const std::vector<std::string> levels = split_list(s->outputLevel);
+  if (levels.size() > OSM_B200_MAX_INPUTS) return hfail(OSM_B200_ERR_UNSUPPORTED, "more than 8 levels in one reader");
+  osm_b200_component c;
+  osm_b200_component_defaults(OSM_B200_C_VECTORCONCAT, &c);
+  // the union of the input levels of several cFunctionals instances keeps every level's own length (graph.cpp: padRows)
+  const char *cname = (s->hasFunc && s->unionLevels.size() > 1) ? "_unionconcat" : "_sinkconcat";
+  snprintf(c.name, sizeof c.name, "%s", cname);
+  for (const std::string &l : levels) snprintf(c.reader_dmLevel[c.n_inputs++], OSM_B200_NAME_LEN, "%s", l.c_str());
+  snprintf(c.writer_dmLevel, sizeof c.writer_dmLevel, "%s", cname);
+  c.u.vectorconcat.processArrayFields = 0;     // a reader's level concatenation keeps every field
+  s->comps.push_back(c);
+  s->outputLevel = cname;
+  return OSM_B200_OK;
+}
+
+// pass 7: validate the graph now (description-only plan at a nominal format) so that errors surface at open
+static osm_b200_status validate(osm_b200_session *s)
+{
+  std::vector<osm_b200_component> cs = s->comps;
+  cs[s->waveIdx].u.wavesource.sampleRate = 16000;
+  cs[s->waveIdx].u.wavesource.nChannels = 1;
+  osm_b200_plan *p = nullptr;
+  osm_b200_status st = osm_b200_plan_create(cs.data(), (int)cs.size(), s->outputLevel.c_str(), -1, &p);
+  const PlanPtr plan(p);
+  if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
+  if (!s->hasFunc) return OSM_B200_OK;
+  // the summary is taken at the first end-of-input tick; how many cTonefilt rows exist then (its last, padded block is
+  // written only after end of input) is not modelled
+  for (const osm_b200_component &c : cs)
+    if (c.type == OSM_B200_C_TONEFILT)
+      return hfail(OSM_B200_ERR_UNSUPPORTED, std::string("cFunctionals reading a level behind cTonefilt '") + c.name + "' is not supported");
+  osm_b200_session::FuncRt rt;
+  return build_func_rt(s, 16000, 1, p, -1, rt);
+}
+
 extern "C" {
 
 // no exception crosses the C boundary (host allocation failures while the configuration is read and lowered)
@@ -1501,320 +1842,17 @@ try {
   int curSec = -1;
   g_herr.clear();
   if (!parse_file(conf_path, s->conf, given, err, curSec)) return hfail(OSM_B200_ERR_INVALID, err);
-  // instances listed in [componentInstances:cComponentManager] (core/componentManager.cpp:840-957)
-  std::map<std::string, const Section *> secOf;
-  for (const auto &sec : s->conf.sections) if (sec.type != "cComponentManager") secOf[sec.name] = &sec;
-  std::vector<std::string> sinkLevels;
   std::vector<const Section *> compute;
-  bool csvLocked = false, arffLocked = false;
-  std::set<std::string> hostTypes = {"cDataMemory", "cHtkSink", "cCsvSink", "cArffSink", "cExternalSink", "cNullSink", "cDatadumpSink"};
-  for (const auto &inst : s->conf.instances) {
-    const std::string &name = inst.first, &type = inst.second;
-    const Section *sec = secOf.count(name) ? secOf[name] : nullptr;
-    if (sec && sec->type != type) return hfail(OSM_B200_ERR_INVALID, "instance '" + name + "' is declared as " + type + " but configured as " + sec->type);
-    if (hostTypes.count(type)) {
-      if (!sec) continue;
-      if (type == "cHtkSink" || type == "cCsvSink" || type == "cArffSink" || type == "cExternalSink") {
-        const std::string *fn = sec->get("filename");
-        const bool active = type == "cExternalSink" || (fn && *fn != "?" && !fn->empty());
-        const std::string *lv = sec->get("reader.dmLevel");
-        if (active && lv) sinkLevels.push_back(*lv);
-        if (type == "cArffSink" && active && !arffLocked) {
-          arffLocked = true;
-          ArffOpts &a = s->arff;
-          a = ArffOpts();
-          if (const std::string *x = sec->get("relation")) a.relation = *x;
-          if (const std::string *x = sec->get("append")) a.append = inum(*x) != 0;
-          if (const std::string *x = sec->get("number")) a.number = inum(*x) == 1;
-          if (const std::string *x = sec->get("frameIndex")) a.number = inum(*x) == 1;
-          if (const std::string *x = sec->get("timestamp")) a.timestamp = inum(*x) == 1;
-          if (const std::string *x = sec->get("frameTime")) a.timestamp = inum(*x) == 1;
-          if (const std::string *x = sec->get("frameTimeAdd")) a.frameTimeAdd = num(*x);
-          if (const std::string *x = sec->get("printDefaultClassDummyAttribute")) a.dummyClass = inum(*x) != 0;
-          if (const std::string *x = sec->get("frameLength")) if (inum(*x) == 1) return hfail(OSM_B200_ERR_UNSUPPORTED, "cArffSink.frameLength=1 is not supported");
-          if (const std::string *x = sec->get("instanceBase")) if (!x->empty() && *x != "-") { a.instName = *x; a.prname = 2; }
-          if (const std::string *x = sec->get("instanceName")) if (!x->empty() && *x != "-") { a.instName = *x; a.prname = 1; }
-          for (int c = 0; c < 64; c++) {                       // class[c].name / class[c].type, target[c].all (:112-170)
-            char key[64];
-            snprintf(key, sizeof key, "class[%d].name", c);
-            const std::string *nm = sec->get(key);
-            snprintf(key, sizeof key, "class[%d].type", c);
-            const std::string *ty = sec->get(key);
-            if (!nm && !ty) break;
-            a.classes.push_back({nm ? *nm : std::string("class"), ty ? *ty : std::string("numeric")});
-            snprintf(key, sizeof key, "target[%d].all", c);
-            const std::string *tg = sec->get(key);
-            a.targetAll.push_back(tg ? (*tg == "?" ? *tg : arff_escape(*tg)) : std::string());
-            snprintf(key, sizeof key, "target[%d].instance[0]", c);
-            if (sec->get(key)) return hfail(OSM_B200_ERR_UNSUPPORTED, "cArffSink.target[].instance[] is not supported");
-          }
-        }
-        if (type == "cHtkSink") { if (const std::string *pk = sec->get("parmKind")) s->parmKind = inum(*pk); }
-        // CSV formatting options: those of the active CSV sink; without one (explicit csv paths over the API),
-        // those of the last cCsvSink section
-        if (type == "cCsvSink" && !csvLocked) {
-          s->csv = CsvOpts();
-          csvLocked = active;
-          if (const std::string *x = sec->get("printHeader")) s->csv.printHeader = inum(*x) != 0;
-          if (const std::string *x = sec->get("timestamp")) s->csv.timestamp = inum(*x) == 1;
-          if (const std::string *x = sec->get("frameTime")) s->csv.timestamp = inum(*x) == 1;
-          if (const std::string *x = sec->get("number")) s->csv.number = inum(*x) == 1;
-          if (const std::string *x = sec->get("frameIndex")) s->csv.number = inum(*x) == 1;
-          if (const std::string *x = sec->get("instanceBase")) { s->csv.instName = *x; s->csv.prname = 2; }
-          if (const std::string *x = sec->get("instanceName")) { s->csv.instName = *x; s->csv.prname = 1; }
-          if (const std::string *x = sec->get("frameLength")) if (inum(*x) == 1) return hfail(OSM_B200_ERR_UNSUPPORTED, "cCsvSink.frameLength=1 is not supported");
-          if (const std::string *x = sec->get("delimChar")) if (!x->empty()) s->csv.delim = *x == "<space>" ? ' ' : (*x == "<tab>" ? '\t' : (*x)[0]);
-        }
-      }
-      continue;
-    }
-    if (!sec) return hfail(OSM_B200_ERR_INVALID, "instance '" + name + "' (" + type + ") has no configuration section");
-    compute.push_back(sec);
-  }
-  // output level: explicit, or the level the active sinks read; a multi-level sink reader is an
-  // implicit concat (core/dataReader.cpp:360-444)
-  std::string lvl = output_level ? output_level : "";
-  if (lvl.empty()) {
-    if (sinkLevels.empty()) return hfail(OSM_B200_ERR_INVALID, "no active sink: pass output_level or enable a sink (-O / -csvoutput)");
-    lvl = sinkLevels[0];
-    // every active sink gets the rows of ONE plan run: sinks that read different levels cannot be served together
-    for (const std::string &l : sinkLevels)
-      if (l != lvl) return hfail(OSM_B200_ERR_UNSUPPORTED, "the active sinks read different levels ('" + lvl + "' and '" + l + "'): enable the sinks of one level per session");
-  }
-  // A summary level: [sink level] <- (single-input cVectorConcat)* <- cFunctionals <- LLD level(s), or several such chains behind
-  // one cVectorConcat / multi-level sink reader.  The plan computes the union of the functionals' input levels; the summaries
-  // run on the resident rows (functionals.cu), each instance on its columns.
-  {
-    std::map<std::string, const Section *> writerOfAll;
-    for (const Section *sec : compute) if (const std::string *w = sec->get("writer.dmLevel")) writerOfAll[*w] = sec;
-    // the summary graph behind the sink: cFunctionals levels below cVectorConcat / cDataSelector / cVectorOperation nodes
-    std::function<bool(const std::string &, int)> has_func = [&](const std::string &cur, int depth) -> bool {
-      auto it = writerOfAll.find(cur);
-      if (it == writerOfAll.end() || depth > 16) return false;
-      const Section *w = it->second;
-      if (w->type == "cFunctionals") return true;
-      if (w->type != "cVectorConcat" && w->type != "cDataSelector" && w->type != "cVectorOperation") return false;
-      const std::string *r = w->get("reader.dmLevel");
-      if (!r) return false;
-      std::vector<std::string> rl;
-      split_levels(*r, rl);
-      for (const std::string &l : rl) if (has_func(l, depth + 1)) return true;
-      return false;
-    };
-    std::string terr;
-    osm_b200_status tst = OSM_B200_ERR_UNSUPPORTED;
-    std::map<const Section *, int> instOf;
-    auto add_inst = [&](const Section *w) -> int {
-      auto it = instOf.find(w);
-      if (it != instOf.end()) return it->second;
-      osm_b200_session::FuncInst fi;
-      if (!to_functionals(*w, fi.spec, terr)) { tst = terr.find("not supported") != std::string::npos ? OSM_B200_ERR_UNSUPPORTED : OSM_B200_ERR_INVALID; return -1; }
-      if (const std::string *x = w->get("preserveFields")) fi.preserveFields = inum(*x) != 0;
-        const std::string *r = w->get("reader.dmLevel");
-        if (!r) { terr = "cFunctionals '" + w->name + "' has no reader.dmLevel"; tst = OSM_B200_ERR_INVALID; return -1; }
-        std::vector<std::string> rl;
-        split_levels(*r, rl);
-        for (const std::string &l : rl) {
-          osm_b200_session::FuncReader rd;
-          rd.level = l;
-          // a cDataSelector that only picks named elements (and appends to their names) is a view of its input level
-          auto itw = writerOfAll.find(l);
-          if (itw != writerOfAll.end() && itw->second->type == "cDataSelector") {
-            const Section *ds = itw->second;
-            bool simple = true;
-            std::map<int, std::string> selIdx;
-            std::string selList;
-            for (const auto &kv : ds->kv) {
-              const std::string &f = kv.first;
-              if (f == "nameAppend") { rd.nameAppend = kv.second; continue; }
-              if (is_common(f) || f == "reader.dmLevel" || f == "writer.dmLevel") continue;
-              if (f == "selected") selList = kv.second;
-              else if (f.compare(0, 9, "selected[") == 0) selIdx[atoi(f.c_str() + 9)] = kv.second;
-              else if (f == "nameAppend") rd.nameAppend = kv.second;
-              else if (f == "elementMode") simple = simple && inum(kv.second) == 1;
-              else if (f == "copyInputName") simple = simple && inum(kv.second) == 1;
-              else simple = false;
-            }
-            const std::string *base = ds->get("reader.dmLevel");
-            if (!selIdx.empty()) for (const auto &kv : selIdx) rd.sel.push_back(trim(kv.second));
-            else split_levels(selList, rd.sel);
-            if (simple && base && base->find(';') == std::string::npos && !rd.sel.empty()) rd.level = trim(*base);
-            else { rd.sel.clear(); rd.nameAppend.clear(); }
-          }
-          fi.readers.push_back(rd);
-          if (std::find(s->unionLevels.begin(), s->unionLevels.end(), rd.level) == s->unionLevels.end()) s->unionLevels.push_back(rd.level);
-        }
-        s->finsts.push_back(fi);
-      instOf[w] = (int)s->finsts.size() - 1;
-      return (int)s->finsts.size() - 1;
-    };
-    std::function<int(const std::string &, int)> build = [&](const std::string &cur, int depth) -> int {
-      auto it = writerOfAll.find(cur);
-      if (it == writerOfAll.end() || depth > 16) { terr = "level '" + cur + "' has no writer"; tst = OSM_B200_ERR_INVALID; return -1; }
-      const Section *w = it->second;
-      osm_b200_session::SummNode nd;
-      if (w->type == "cFunctionals") {
-        nd.kind = 0;
-        nd.inst = add_inst(w);
-        if (nd.inst < 0) return -1;
-        s->snodes.push_back(nd);
-        return (int)s->snodes.size() - 1;
-      }
-      const std::string *r = w->get("reader.dmLevel");
-      if (!r || (w->type != "cVectorConcat" && w->type != "cDataSelector" && w->type != "cVectorOperation")) {
-        terr = "a level that mixes cFunctionals summaries with other levels is not supported (level '" + cur + "')"; tst = OSM_B200_ERR_UNSUPPORTED; return -1;
-      }
-      std::vector<std::string> rl;
-      split_levels(*r, rl);
-      for (const std::string &l : rl) { const int k = build(l, depth + 1); if (k < 0) return -1; nd.kids.push_back(k); }
-      if (w->type == "cVectorConcat") {
-        // summary levels hold single-element fields: a cVectorConcat that keeps only array fields (its default) would be empty
-        nd.kind = 1;
-        int paf = 1, incl = 0;
-        if (const std::string *x = w->get("processArrayFields")) paf = inum(*x);
-        if (const std::string *x = w->get("includeSingleElementFields")) incl = inum(*x);
-        if (paf == 1 && !incl && rl.size() > 1) { terr = "cVectorConcat '" + w->name + "' behind cFunctionals drops single-element fields (includeSingleElementFields = 0)"; tst = OSM_B200_ERR_UNSUPPORTED; return -1; }
-      } else if (w->type == "cDataSelector") {
-        nd.kind = 2;
-        std::map<int, std::string> selIdx, newIdx;
-        std::string selList, newList;
-        for (const auto &kv : w->kv) {
-          const std::string &f = kv.first;
-          if (f == "nameAppend") { nd.nameAppend = kv.second; continue; }
-          if (is_common(f) || f == "reader.dmLevel" || f == "writer.dmLevel") continue;
-          if (f == "selected") selList = kv.second;
-          else if (f.compare(0, 9, "selected[") == 0) selIdx[atoi(f.c_str() + 9)] = kv.second;
-          else if (f == "newNames") newList = kv.second;
-          else if (f.compare(0, 9, "newNames[") == 0) newIdx[atoi(f.c_str() + 9)] = kv.second;
-          else if (f == "elementMode") { if (inum(kv.second) != 1) { terr = "cDataSelector.elementMode=0 is not supported"; return -1; } }
-          else if (f == "copyInputName") { if (inum(kv.second) != 1) { terr = "cDataSelector.copyInputName=0 is not supported"; return -1; } }
-          else { terr = "cDataSelector '" + w->name + "': field '" + f + "' is not supported"; return -1; }
-        }
-        if (!selIdx.empty()) for (const auto &kv : selIdx) nd.sel.push_back(trim(kv.second)); else split_levels(selList, nd.sel);
-        if (!newIdx.empty()) { nd.newNames.assign(nd.sel.size(), ""); for (const auto &kv : newIdx) if (kv.first >= 0 && (size_t)kv.first < nd.newNames.size()) nd.newNames[(size_t)kv.first] = trim(kv.second); }
-        else split_levels(newList, nd.newNames);
-        if (nd.sel.empty()) { terr = "cDataSelector '" + w->name + "': no elements selected"; tst = OSM_B200_ERR_INVALID; return -1; }
-      } else {
-        nd.kind = 3;                                                  // other/vectorOperation.cpp:42-48,136-139,210-222
-        std::string opn = "norm";
-        int appendOp = 0;
-        double lf = 1e-12;                                            // default of `logfloor`
-        for (const auto &kv : w->kv) {
-          const std::string &f = kv.first;
-          if (f == "nameAppend") { nd.nameAppend = kv.second; continue; }
-          if (f == "copyInputName") { nd.copyInputName = inum(kv.second) != 0; continue; }
-          if (is_common(f) || f == "reader.dmLevel" || f == "writer.dmLevel") continue;
-          if (f == "operation") opn = kv.second;
-          else if (f == "nameBase") nd.nameBase = kv.second;
-          else if (f == "appendOperationToName") appendOp = inum(kv.second);
-          else if (f == "logfloor") lf = atof(kv.second.c_str());
-          else if (f == "processArrayFields" || f == "includeSingleElementFields" || f == "param1" || f == "param2" || f == "powOnlyPos") continue;
-          else { terr = "cVectorOperation '" + w->name + "': field '" + f + "' is not supported"; return -1; }
-        }
-        if (opn.compare(0, 3, "dBp") == 0) nd.op = OSM_B200_VOP_DBP;
-        else if (opn.compare(0, 3, "dBv") == 0) nd.op = OSM_B200_VOP_DBV;
-        else { terr = "cVectorOperation behind cFunctionals: only operation = dBp / dBv is supported (got '" + opn + "')"; return -1; }
-        if (appendOp) nd.nameAppend = opn;                             // overrides nameAppend (:210-216, :240-243)
-        if (lf <= 0) lf = 0.000000000001;                              // :219-223
-        nd.logfloor = (float)lf;
-        if (rl.size() != 1) { terr = "cVectorOperation must read exactly one level"; return -1; }
-      }
-      s->snodes.push_back(nd);
-      return (int)s->snodes.size() - 1;
-    };
-    std::vector<std::string> parts;
-    split_levels(lvl, parts);
-    bool anyFunc = false;
-    for (const std::string &pl : parts) anyFunc = anyFunc || has_func(pl, 0);
-    if (anyFunc) {
-      if (parts.size() == 1) s->sroot = build(parts[0], 0);
-      else {
-        osm_b200_session::SummNode root;
-        root.kind = 1;
-        bool ok = true;
-        for (const std::string &pl : parts) { const int k = build(pl, 0); if (k < 0) { ok = false; break; } root.kids.push_back(k); }
-        if (ok) { s->snodes.push_back(root); s->sroot = (int)s->snodes.size() - 1; }
-      }
-      if (s->sroot < 0) return hfail(tst, terr);
-      if (s->unionLevels.size() > OSM_B200_MAX_INPUTS) return hfail(OSM_B200_ERR_UNSUPPORTED, "cFunctionals: more than 8 input levels in total");
-      s->hasFunc = true;
-      lvl.clear();
-      for (const std::string &l : s->unionLevels) lvl += (lvl.empty() ? "" : ";") + l;
-    }
-  }
-  // Only the components the output level depends on are part of the plan: the shipped feature-set
-  // configurations carry sinks and summaries (cFunctionals ...) that stay idle when their output file is
-  // not requested (filename = ?), exactly like the reference leaves those sinks unwritten.
-  {
-    std::map<std::string, const Section *> writerOf;
-    for (const Section *sec : compute) if (const std::string *w = sec->get("writer.dmLevel")) writerOf[*w] = sec;
-    std::set<const Section *> need;
-    std::vector<std::string> todo;
-    auto push_levels = [&](const std::string &v) {
-      std::stringstream ss(v);
-      std::string one;
-      while (std::getline(ss, one, ';')) { one = trim(one); if (!one.empty()) todo.push_back(one); }
-    };
-    push_levels(lvl);
-    while (!todo.empty()) {
-      const std::string l = todo.back();
-      todo.pop_back();
-      auto it = writerOf.find(l);
-      if (it == writerOf.end() || need.count(it->second)) continue;
-      need.insert(it->second);
-      for (const char *key : {"reader.dmLevel", "reader2.dmLevel", "F0reader.dmLevel"})
-        if (const std::string *r = it->second->get(key)) push_levels(*r);
-    }
-    for (const Section *sec : compute) {
-      const bool isWave = sec->type == "cWaveSource" || sec->type == "cExternalAudioSource";
-      if (!isWave && !need.count(sec)) continue;
-      osm_b200_component c;
-      if (!to_component(*sec, c, err)) {
-        return hfail(type_of(sec->type) < 0 ? OSM_B200_ERR_UNSUPPORTED : OSM_B200_ERR_INVALID, err);
-      }
-      if (c.type == OSM_B200_C_WAVESOURCE) s->waveIdx = (int)s->comps.size();
-      s->comps.push_back(c);
-    }
-  }
-  if (s->waveIdx < 0) return hfail(OSM_B200_ERR_INVALID, "the configuration has no cWaveSource / cExternalAudioSource");
-  if (lvl.find(';') != std::string::npos) {
-    osm_b200_component c;
-    osm_b200_component_defaults(OSM_B200_C_VECTORCONCAT, &c);
-    // the union of the input levels of several cFunctionals instances keeps every level's own length (graph.cpp: padRows)
-    const char *cname = (s->hasFunc && s->unionLevels.size() > 1) ? "_unionconcat" : "_sinkconcat";
-    snprintf(c.name, sizeof c.name, "%s", cname);
-    std::stringstream ss(lvl);
-    std::string one;
-    while (std::getline(ss, one, ';')) {
-      one = trim(one);
-      if (!one.empty() && c.n_inputs < OSM_B200_MAX_INPUTS) snprintf(c.reader_dmLevel[c.n_inputs++], OSM_B200_NAME_LEN, "%s", one.c_str());
-    }
-    snprintf(c.writer_dmLevel, sizeof c.writer_dmLevel, "%s", cname);
-    c.u.vectorconcat.processArrayFields = 0;     // a reader's level concatenation keeps every field
-    s->comps.push_back(c);
-    lvl = cname;
-  }
-  s->outputLevel = lvl;
-  // validate the graph now (description-only plan at a nominal format) so that errors surface at open
-  {
-    std::vector<osm_b200_component> cs = s->comps;
-    cs[s->waveIdx].u.wavesource.sampleRate = 16000;
-    cs[s->waveIdx].u.wavesource.nChannels = 1;
-    osm_b200_plan *p = nullptr;
-    osm_b200_status st = osm_b200_plan_create(cs.data(), (int)cs.size(), s->outputLevel.c_str(), -1, &p);
-    const PlanPtr plan(p);
-    if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
-    if (s->hasFunc) {
-      // the summary is taken at the first end-of-input tick; how many cTonefilt rows exist then (its last, padded block is
-      // written only after end of input) is not modelled
-      for (const osm_b200_component &c : cs)
-        if (c.type == OSM_B200_C_TONEFILT)
-          return hfail(OSM_B200_ERR_UNSUPPORTED, std::string("cFunctionals reading a level behind cTonefilt '") + c.name + "' is not supported");
-      osm_b200_session::FuncRt rt;
-      st = build_func_rt(s.get(), 16000, 1, p, -1, rt);
-      if (st != OSM_B200_OK) return hfail(st, osm_b200_host_last_error());
-    }
-  }
+  std::vector<std::string> sinkLevels;
+  osm_b200_status st = read_instances(s.get(), compute, sinkLevels);
+  if (st == OSM_B200_OK) st = choose_output_level(output_level, sinkLevels, s->outputLevel);
+  std::map<std::string, const Section *> writerOf;
+  for (const Section *sec : compute) if (const std::string *w = sec->get("writer.dmLevel")) writerOf[*w] = sec;
+  if (st == OSM_B200_OK) st = build_summary(s.get(), writerOf);
+  if (st == OSM_B200_OK) st = lower_sections(s.get(), compute, writerOf);
+  if (st == OSM_B200_OK) st = add_reader_concat(s.get());
+  if (st == OSM_B200_OK) st = validate(s.get());
+  if (st != OSM_B200_OK) return st;
   *session = s.release();
   return OSM_B200_OK;
 } catch (const std::bad_alloc &) { return hfail(OSM_B200_ERR_NOMEM, "out of host memory"); }
@@ -1900,7 +1938,6 @@ static osm_b200_status osm_b200_session_extract_pcm_impl(osm_b200_session *s, co
         const int64_t n = std::min<int64_t>(osm_b200_plan_num_frames_first_eoi(f->desc[i] ? f->desc[i].get() : p, uttOff[u + 1] - uttOff[u]), lldOff[u + 1] - lldOff[u]);
         nRows[i][live.size()] = n;
         all = all && n > 0;
-        if (getenv("OSM_B200_DEBUG_FUNC")) fprintf(stderr, "functionals instance %zu: utterance %d sees %lld rows (level rows %lld)\n", i, u, (long long)n, (long long)(lldOff[u + 1] - lldOff[u]));
       }
       if (all) { rowOff[live.size()] = lldOff[u]; live.push_back(u); }
       frameOff[u + 1] = frameOff[u] + (all ? 1 : 0);
@@ -1909,10 +1946,6 @@ static osm_b200_status osm_b200_session_extract_pcm_impl(osm_b200_session *s, co
     if (frameOff[nUtt] > maxRows) return hfail(OSM_B200_ERR_INVALID, "output buffer too small");
     if (live.empty()) return OSM_B200_OK;
     const float *dRows = nullptr;
-    const bool timing = getenv("OSM_B200_FUNC_TIMING") != nullptr;       // dev aid: host wall clock of the phases, to stderr
-    auto now = [] { return std::chrono::steady_clock::now(); };
-    auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
-    const auto t0 = now();
     if (dev) {
       if (s->dLldRows.reserve((size_t)lldOff[(size_t)nUtt] * osm_b200_plan_num_elements(p)) != cudaSuccess)
         return hfail(OSM_B200_ERR_NOMEM, "out of device memory (LLD rows)");
@@ -1923,8 +1956,6 @@ static osm_b200_status osm_b200_session_extract_pcm_impl(osm_b200_session *s, co
       st = osm_b200_plan_run_host_resident(p, pcm, uttOff, nUtt, lldOff.data(), &dRows);
     }
     if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
-    if (timing) cudaStreamSynchronize(stream);
-    const auto t1 = now();
     // levels behind the SHS pitch chain: their length at the first end-of-input tick follows the Viterbi level's (data dependent)
     {
       std::vector<int32_t> lag((size_t)nUtt, -1);
@@ -1938,7 +1969,6 @@ static osm_b200_status osm_b200_session_extract_pcm_impl(osm_b200_session *s, co
                                                                lldOff[u + 1] - lldOff[u]));
       }
     }
-    const auto t2 = now();
     const int KF = f->total, KS = f->scratch;
     const size_t need = live.size() * (size_t)KF;
     float *dInst = nullptr;                                            // where the instances write: the sink's row or the scratch row
@@ -1962,11 +1992,7 @@ static osm_b200_status osm_b200_session_extract_pcm_impl(osm_b200_session *s, co
       st = osm_b200_summary_assemble_device(dInst, KS, f->gSrc.data(), f->gOp.data(), f->gFloor.data(), KF, (int64_t)live.size(), dSink, KF, stream);
       if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
     }
-    if (timing) cudaStreamSynchronize(stream);
-    const auto t3 = now();
     if (!dev && cudaMemcpy(out, s->dFuncOut.p, need * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess) return hfail(OSM_B200_ERR_CUDA, "copy of the functionals rows failed");
-    if (timing) fprintf(stderr, "summary timing: LLD plan (H2D + kernels) %.2f ms, row counts %.2f ms, %zu cFunctionals instances + assemble %.2f ms, D2H %.2f ms\n",
-                        ms(t0, t1), ms(t1, t2), nI, ms(t2, t3), ms(t3, now()));
     return OSM_B200_OK;
   }
   st = osm_b200_plan_frame_offsets(p, uttOff, nUtt, frameOff);
@@ -2143,52 +2169,55 @@ try {
     osm_b200_plan *p;
     osm_b200_status st = get_plan(s, sr, nc, &p, fmt);
     if (st != OSM_B200_OK) return st;
+    const int nG = (int)g.second.size();
+    int K = 0;
+    std::vector<float> rows;
+    std::vector<std::string> names;
+    // Device sinks (sinks.cu): the rows stay in HBM after the plan run, the CSV value text and the HTK payload are produced there
+    // and copied next to the float rows; the host threads add the per-row prefixes and write.  OSM_B200_DEVICE_SINKS=0: host formatting.
+    static const bool devSinks = [] { const char *e = getenv("OSM_B200_DEVICE_SINKS"); return !(e && e[0] == '0'); }();
+    const bool wantCsv = csvPaths != nullptr, wantHtk = htkPaths != nullptr, wantArff = arffPaths != nullptr;
+    bool devText = false;
+    HostText csv, arff;                                     // cArffSink: every value "%e", ',' between them (iocore/arffSink.cpp:300-312)
+    std::vector<uint32_t> packed;
     if (s->hasFunc) {
       // a summary configuration (cFunctionals behind the sink's level): one row per input that has frames, as the reference's sinks
       // write it -- instance name, time stamp 0 (the summary's segment starts at 0), the values
       osm_b200_session::FuncRt *f;
       st = get_func(s, sr, nc, p, &f);
       if (st != OSM_B200_OK) return st;
-      const int KF = f->total;
-      std::vector<float> frows(g.second.size() * (size_t)KF + 1);
-      st = osm_b200_session_extract_pcm_impl(s, pcm.data(), off.data(), (int)g.second.size(), sr, nc, fo.data(), frows.data(), (int64_t)g.second.size(), fmt);
+      K = f->total;
+      names = f->names;
+      rows.resize((size_t)nG * K + 1);
+      st = osm_b200_session_extract_pcm_impl(s, pcm.data(), off.data(), nG, sr, nc, fo.data(), rows.data(), nG, fmt);
       if (st != OSM_B200_OK) return st;
-      for (size_t k = 0; k < g.second.size(); k++) nTime[k] = fo[k + 1] - fo[k];
-      if (!write_batch(s, g.second, fo.data(), nTime.data(), frows.data(), KF, f->names, osm_b200_plan_frame_period(p), htkPaths, csvPaths, arffPaths, framesOut, err))
-        return hfail(OSM_B200_ERR_INVALID, err);
-      continue;
-    }
-    st = osm_b200_plan_frame_offsets(p, off.data(), (int)g.second.size(), fo.data());
-    if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
-    const int K = osm_b200_plan_num_elements(p);
-    const int64_t nR = fo.back();
-    std::vector<float> rows((size_t)nR * K + 1);
-    std::vector<std::string> names(K);
-    for (int k = 0; k < K; k++) names[k] = osm_b200_plan_element_name(p, k);
-    for (size_t k = 0; k < g.second.size(); k++) nTime[k] = osm_b200_plan_num_time_frames(p, off[k + 1] - off[k]);
-    // Device sinks (sinks.cu): the rows stay in HBM after the plan run, the CSV value text and the HTK payload are produced there
-    // and copied next to the float rows; the host threads add the per-row prefixes and write.  OSM_B200_DEVICE_SINKS=0: host formatting.
-    static const bool devSinks = [] { const char *e = getenv("OSM_B200_DEVICE_SINKS"); return !(e && e[0] == '0'); }();
-    const bool wantCsv = csvPaths != nullptr, wantHtk = htkPaths != nullptr, wantArff = arffPaths != nullptr;
-    if (devSinks && nR > 0 && (wantCsv || wantHtk || wantArff)) {
-      const float *dRows = nullptr;
-      st = osm_b200_plan_run_host_resident(p, pcm.data(), off.data(), (int)g.second.size(), fo.data(), &dRows);
+      for (int k = 0; k < nG; k++) nTime[k] = fo[k + 1] - fo[k];
+    } else {
+      st = osm_b200_plan_frame_offsets(p, off.data(), nG, fo.data());
       if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
-      HostText csv, arff;                                   // cArffSink: every value "%e", ',' between them (iocore/arffSink.cpp:300-312)
-      std::vector<uint32_t> packed;
-      const bool ok = cudaMemcpy(rows.data(), dRows, (size_t)nR * K * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess &&
-                      (!wantCsv || device_text(dRows, nR, K, s->csv.delim, false, csv)) &&
-                      (!wantArff || device_text(dRows, nR, K, ',', true, arff)) && (!wantHtk || device_htk(dRows, nR, K, packed));
-      if (!ok) return hfail(OSM_B200_ERR_CUDA, std::string("device sinks: ") + cudaGetErrorString(cudaGetLastError()));
-      const DevText dt = csv.view(), dtA = arff.view();
-      if (!write_batch(s, g.second, fo.data(), nTime.data(), rows.data(), K, names, osm_b200_plan_frame_period(p), htkPaths, csvPaths, arffPaths, framesOut, err,
-                       wantCsv ? &dt : nullptr, wantHtk ? packed.data() : nullptr, wantArff ? &dtA : nullptr))
-        return hfail(OSM_B200_ERR_INVALID, err);
-      continue;
+      K = osm_b200_plan_num_elements(p);
+      const int64_t nR = fo.back();
+      rows.resize((size_t)nR * K + 1);
+      names.resize(K);
+      for (int k = 0; k < K; k++) names[k] = osm_b200_plan_element_name(p, k);
+      for (int k = 0; k < nG; k++) nTime[k] = osm_b200_plan_num_time_frames(p, off[k + 1] - off[k]);
+      devText = devSinks && nR > 0 && (wantCsv || wantHtk || wantArff);
+      if (devText) {
+        const float *dRows = nullptr;
+        st = osm_b200_plan_run_host_resident(p, pcm.data(), off.data(), nG, fo.data(), &dRows);
+        if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
+        const bool ok = cudaMemcpy(rows.data(), dRows, (size_t)nR * K * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess &&
+                        (!wantCsv || device_text(dRows, nR, K, s->csv.delim, false, csv)) &&
+                        (!wantArff || device_text(dRows, nR, K, ',', true, arff)) && (!wantHtk || device_htk(dRows, nR, K, packed));
+        if (!ok) return hfail(OSM_B200_ERR_CUDA, std::string("device sinks: ") + cudaGetErrorString(cudaGetLastError()));
+      } else {
+        st = osm_b200_plan_run_host(p, pcm.data(), off.data(), nG, fo.data(), rows.data());
+        if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
+      }
     }
-    st = osm_b200_plan_run_host(p, pcm.data(), off.data(), (int)g.second.size(), fo.data(), rows.data());
-    if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
-    if (!write_batch(s, g.second, fo.data(), nTime.data(), rows.data(), K, names, osm_b200_plan_frame_period(p), htkPaths, csvPaths, arffPaths, framesOut, err))
+    const DevText dt = csv.view(), dtA = arff.view();
+    if (!write_batch(s, g.second, fo.data(), nTime.data(), rows.data(), K, names, osm_b200_plan_frame_period(p), htkPaths, csvPaths, arffPaths, framesOut, err,
+                     devText && wantCsv ? &dt : nullptr, devText && wantHtk ? packed.data() : nullptr, devText && wantArff ? &dtA : nullptr))
       return hfail(OSM_B200_ERR_INVALID, err);
   }
   return OSM_B200_OK;
@@ -2293,16 +2322,7 @@ int32_t osm_b200_write_htk(const char *path, const float *rows, int64_t n, int32
 int32_t osm_b200_write_csv(const char *path, const float *rows, int64_t n, int32_t K, const char *const *names, double period,
                            const char *instName, int32_t frameIndex, int32_t frameTime)
 {
-  std::string err;
-  std::vector<std::string> nm(K);
-  for (int k = 0; k < K; k++) nm[k] = names[k];
-  CsvOpts o;
-  if (instName) { o.instName = instName; o.prname = 1; }
-  o.number = frameIndex != 0;
-  o.timestamp = frameTime != 0;
-  if (write_csv(path, rows, n, K, nm, period, o, err)) return 0;
-  g_herr = err;
-  return 1;
+  return osm_b200_write_csv_timed(path, rows, n, K, names, period, instName, frameIndex, frameTime, 0);
 }
 
 int32_t osm_b200_write_csv_timed(const char *path, const float *rows, int64_t n, int32_t K, const char *const *names, double period,

@@ -39,8 +39,6 @@ for lv in levels:
         bad = [(names[c], float(worst[c]), int(np.argmax(err[:, c]))) for c in range(len(names)) if worst[c] > 1e-4]
         print("LEVEL", lv, k, got.shape, "max err/scale %.2e" % worst.max(), bad[:6])
 for tag, cf in (("egemaps", "egemaps/v02/eGeMAPSv02.conf"), ("gemaps", "gemaps/v01b/GeMAPSv01b.conf")):
-    os.environ["OSM_B200_DEBUG_FUNC"] = "1" if tag == "egemaps" else ""
-    if not os.environ["OSM_B200_DEBUG_FUNC"]: del os.environ["OSM_B200_DEBUG_FUNC"]
     s = Session(os.path.join(REFCONF, cf), options={"csvoutput": "f.csv"}, device=0)
     names = s.element_names()
     rows, fo = s.extract_pcm(allpcm, off, 16000.0, 1)

@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 
 from conftest import ROOT
-from opensmile_b200 import Session, SessionError, capi, write_csv, write_htk
+from opensmile_b200 import Session, SessionError, capi, write_arff, write_csv, write_htk
 
 CONF = os.path.join(ROOT, "tests", "configs")
 GOLD = np.load(os.path.join(ROOT, "tests", "golden", "conf_goldens.npz"))
@@ -310,3 +310,13 @@ def test_partial_file_options_are_refused_not_ignored():
             Session(conf, options=dict(opts, O="x.htk"), device=-1)
         assert e.value.status == capi.ERR_UNSUPPORTED or e.value.status == capi.ERR_INVALID
         assert needle in str(e.value)
+
+
+@pytest.mark.skipif(not os.path.exists("/dev/full"), reason="no /dev/full on this system")
+def test_text_and_htk_writers_report_a_failed_write():
+    """a write that fails (every write to /dev/full ends in ENOSPC) is an error of each writer, not a silently short file"""
+    rows = np.arange(6, dtype=np.float32).reshape(3, 2)
+    for write in (lambda: write_htk("/dev/full", rows, 0.01), lambda: write_csv("/dev/full", rows, ["a", "b"], 0.01),
+                  lambda: write_arff("/dev/full", rows, ["a", "b"], 0.01)):
+        with pytest.raises(IOError, match="write error on '/dev/full'"):
+            write()
