@@ -103,6 +103,30 @@ OSM_B200_API osm_b200_status osm_b200_session_extract_device(osm_b200_session *s
                                                              int64_t *frame_offsets_out, float *d_out, int64_t max_rows,
                                                              void *stream);
 
+/* A session whose active sinks read two levels, one a summary level (cFunctionals, possibly behind cVectorConcat / cDataSelector /
+ * cVectorOperation) and one not (e.g. -csvoutput with -lldcsvoutput of the shipped feature sets), serves both from one plan run: its
+ * output level is the summary, and it has an LLD part, the rows the LLD sinks read.  Any other mix of levels is refused at open.
+ *   osm_b200_session_lld_num_elements / _lld_element_name: the LLD part's elements for an input format (0 / NULL without one); the
+ *       names are those of a session with the LLD sinks alone
+ *   osm_b200_session_extract_device_lld: osm_b200_session_extract_device, also filling lld_frame_offsets_out (n_utt + 1 entries, the
+ *       row counts of a session with the LLD sinks alone) and, when d_out or d_lld_out is not NULL, d_lld_out (DEVICE, at least
+ *       max_lld_rows * lld_num_elements floats; NULL is accepted when the LLD part has no rows) with the LLD rows
+ *   osm_b200_session_extract_files_lld: osm_b200_session_extract_files_arff, also writing the LLD sinks' files (lld_*_paths, with the
+ *       options of the sinks that read the LLD level); LLD paths on a session without an LLD part are an error */
+OSM_B200_API int32_t osm_b200_session_lld_num_elements(osm_b200_session *session, double sample_rate, int32_t n_channels);
+OSM_B200_API const char *osm_b200_session_lld_element_name(osm_b200_session *session, int32_t idx);
+OSM_B200_API osm_b200_status osm_b200_session_extract_device_lld(osm_b200_session *session, const void *d_pcm, int32_t pcm_format,
+                                                                 int64_t stride, const int64_t *lengths, int32_t n_utt,
+                                                                 double sample_rate, int32_t n_channels,
+                                                                 int64_t *frame_offsets_out, float *d_out, int64_t max_rows,
+                                                                 int64_t *lld_frame_offsets_out, float *d_lld_out, int64_t max_lld_rows,
+                                                                 void *stream);
+OSM_B200_API osm_b200_status osm_b200_session_extract_files_lld(osm_b200_session *session, int32_t n, const char *const *wav_paths,
+                                                                const char *const *htk_paths, const char *const *csv_paths,
+                                                                const char *const *arff_paths, const char *const *lld_htk_paths,
+                                                                const char *const *lld_csv_paths, const char *const *lld_arff_paths,
+                                                                int64_t *frames_out);
+
 /* the component list the session resolved (for diagnostics / tests): number of osm_b200_component
  * entries and a pointer to them (owned by the session, valid until close) */
 OSM_B200_API int32_t osm_b200_session_components(osm_b200_session *session, double sample_rate, int32_t n_channels,
@@ -150,6 +174,10 @@ OSM_B200_API int32_t osm_b200_device_format_csv(const float *d_rows, int64_t n_r
 OSM_B200_API int32_t osm_b200_device_format_rows(const float *d_rows, int64_t n_rows, int32_t n_elements, char delim, int32_t always_e,
                                                  char *d_text, int64_t slot_bytes, int32_t *d_row_len, uint8_t *d_row_host, void *stream);
 OSM_B200_API int32_t osm_b200_device_pack_htk(const float *d_rows, int64_t n_values, uint32_t *d_out, void *stream);
+/*   osm_b200_device_gather_rows: d_out[r][k] = d_in[src_off[u] + r - dst_off[u]][cols[k]] for dst_off[u] <= r < dst_off[u + 1]; d_meta is
+ *       one device array {cols[n_cols], src_off[n_utt], dst_off[n_utt + 1]}, n_out_rows = dst_off[n_utt] */
+OSM_B200_API int32_t osm_b200_device_gather_rows(const float *d_in, int32_t in_stride, const int64_t *d_meta, int32_t n_cols, int32_t n_utt,
+                                                 int64_t n_out_rows, float *d_out, void *stream);
 /* whole files from device rows (format on the device, copy, write): byte-identical to osm_b200_write_csv_timed / osm_b200_write_htk */
 OSM_B200_API int32_t osm_b200_write_csv_device(const char *path, const float *d_rows, int64_t n_rows, int32_t n_elements,
                                                const char *const *names, double period, const char *instance_name,

@@ -291,7 +291,7 @@ EXPORTS = [
     # include/osm_b200_functionals.h
     "osm_b200_functionals_defaults", "osm_b200_functionals_create", "osm_b200_functionals_destroy", "osm_b200_functionals_num_values",
     "osm_b200_functionals_num_elements", "osm_b200_functionals_element_name", "osm_b200_functionals_run_device", "osm_b200_functionals_run_device_cols", "osm_b200_summary_assemble_device", "osm_b200_plan_sample_frame_bytes", "osm_b200_device_csv_slot_bytes", "osm_b200_device_format_csv", "osm_b200_device_format_rows",
-    "osm_b200_device_pack_htk", "osm_b200_write_csv_device", "osm_b200_write_htk_device", "osm_b200_functionals_run_host",
+    "osm_b200_device_pack_htk", "osm_b200_device_gather_rows", "osm_b200_write_csv_device", "osm_b200_write_htk_device", "osm_b200_functionals_run_host",
     "osm_b200_functionals_sizeof_spec",
     "osm_b200_plan_last_launch_count", "osm_b200_plan_take_device_flags", "osm_b200_plan_last_kernel_ms",
     "osm_b200_plan_last_kernel_times", "osm_b200_plan_set_profiling", "osm_b200_plan_profile_count", "osm_b200_plan_profile_entry",
@@ -300,7 +300,8 @@ EXPORTS = [
     "osm_b200_session_open", "osm_b200_session_close", "osm_b200_session_num_elements",
     "osm_b200_session_element_name", "osm_b200_session_extract_files", "osm_b200_session_extract_files_arff", "osm_b200_session_sink_options",
     "osm_b200_session_write_files",
-    "osm_b200_session_extract_pcm", "osm_b200_session_extract_device", "osm_b200_session_components", "osm_b200_session_plan", "osm_b200_host_last_error",
+    "osm_b200_session_extract_pcm", "osm_b200_session_extract_device", "osm_b200_session_extract_device_lld", "osm_b200_session_extract_files_lld",
+    "osm_b200_session_lld_num_elements", "osm_b200_session_lld_element_name", "osm_b200_session_components", "osm_b200_session_plan", "osm_b200_host_last_error",
     "osm_b200_write_htk", "osm_b200_write_csv", "osm_b200_write_csv_timed", "osm_b200_write_arff",
 ]
 
@@ -374,6 +375,11 @@ def lib():
     L.osm_b200_session_write_files.restype = i32
     L.osm_b200_session_extract_pcm.argtypes = [vp, vp, i64p, i32, f64, i32, i64p, vp, C.c_int64]
     L.osm_b200_session_extract_device.argtypes = [vp, vp, i32, C.c_int64, i64p, i32, f64, i32, i64p, vp, C.c_int64, vp]
+    L.osm_b200_session_extract_device_lld.argtypes = [vp, vp, i32, C.c_int64, i64p, i32, f64, i32, i64p, vp, C.c_int64, i64p, vp, C.c_int64, vp]
+    L.osm_b200_session_extract_files_lld.argtypes = [vp, i32, cpp, cpp, cpp, cpp, cpp, cpp, cpp, i64p]
+    L.osm_b200_session_lld_num_elements.argtypes = [vp, f64, i32]
+    L.osm_b200_session_lld_element_name.argtypes = [vp, i32]
+    L.osm_b200_session_lld_element_name.restype = C.c_char_p
     L.osm_b200_session_components.argtypes = [vp, f64, i32, C.POINTER(C.POINTER(Component)), cpp]
     L.osm_b200_host_last_error.restype = C.c_char_p
     L.osm_b200_write_htk.argtypes = [C.c_char_p, vp, C.c_int64, i32, f64, i32]

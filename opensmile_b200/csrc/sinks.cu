@@ -8,6 +8,8 @@
 //             values) are flagged and formatted by the host writer.
 //   cArffSink (iocore/arffSink.cpp:300-312): every value "%e", ',' between them -> the same kernel with alwaysE (integers >= 1e7 go to
 //             the host writer as well)
+// gather_rows_kernel picks an LLD sink's columns and rows out of the union level a summary configuration's plan leaves in HBM, into
+// the packed [rows][columns] layout the two kernels above read (a session whose sinks read a summary and an LLD level).
 #include <cuda_runtime.h>
 
 #include "../../include/osm_b200_host.h"
@@ -55,6 +57,21 @@ __global__ void htk_pack_kernel(const uint32_t *__restrict__ in, uint32_t *__res
   if (i < n) out[i] = __byte_perm(in[i], 0, 0x0123);
 }
 
+// one warp per output row: row r of utterance u (dstOff[u] <= r < dstOff[u + 1]) is row srcOff[u] + r - dstOff[u] of `in`, columns
+// cols[0 .. nCols); a copy, no arithmetic
+__global__ void __launch_bounds__(kSinkWarps * 32) gather_rows_kernel(const float *__restrict__ in, int inStride, const long long *__restrict__ cols,
+                                                                       int nCols, const long long *__restrict__ srcOff,
+                                                                       const long long *__restrict__ dstOff, int nUtt, float *__restrict__ out)
+{
+  const long long r = (long long)blockIdx.x * kSinkWarps + (threadIdx.x >> 5);
+  if (r >= dstOff[nUtt]) return;
+  int lo = 0, hi = nUtt - 1;                          // the last u with dstOff[u] <= r
+  while (lo < hi) { const int m = (lo + hi + 1) >> 1; if (dstOff[m] <= r) lo = m; else hi = m - 1; }
+  const float *src = in + (srcOff[lo] + r - dstOff[lo]) * inStride;
+  float *dst = out + r * nCols;
+  for (int k = threadIdx.x & 31; k < nCols; k += 32) dst[k] = src[cols[k]];
+}
+
 }  // namespace
 }  // namespace osm
 
@@ -87,6 +104,18 @@ int32_t osm_b200_device_pack_htk(const float *d_rows, int64_t n_values, uint32_t
   if (!d_rows || !d_out) return 1;
   const long long blocks = (n_values + 255) / 256;
   htk_pack_kernel<<<(unsigned)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(reinterpret_cast<const uint32_t *>(d_rows), d_out, n_values);
+  return cudaGetLastError() == cudaSuccess ? 0 : 2;
+}
+
+int32_t osm_b200_device_gather_rows(const float *d_in, int32_t in_stride, const int64_t *d_meta, int32_t n_cols, int32_t n_utt,
+                                    int64_t n_out_rows, float *d_out, void *stream)
+{
+  if (n_out_rows <= 0) return 0;
+  if (!d_in || !d_meta || !d_out || n_cols <= 0 || n_utt <= 0) return 1;
+  const long long *meta = reinterpret_cast<const long long *>(d_meta);
+  const long long blocks = (n_out_rows + kSinkWarps - 1) / kSinkWarps;
+  gather_rows_kernel<<<(unsigned)blocks, kSinkWarps * 32, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      d_in, in_stride, meta, n_cols, meta + n_cols, meta + n_cols + n_utt, n_utt, d_out);
   return cudaGetLastError() == cudaSuccess ? 0 : 2;
 }
 

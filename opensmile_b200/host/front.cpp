@@ -1290,6 +1290,10 @@ struct osm_b200_session {
     int total = 0;
     bool identity = true;                    // the sink's row is the scratch row
     std::vector<int32_t> gSrc, gOp; std::vector<float> gFloor;
+    PlanPtr sum;                             // with an LLD part: the summary's own plan description (frame counts, period); null = the main plan
+    PlanPtr lld;                             // the LLD part's plan description (its row counts, names, period, time stamps); null = none
+    std::vector<int64_t> lldCols;            // its columns inside the plan's rows
+    std::vector<std::string> lldNames;
   };
   std::map<std::pair<long, int>, FuncRt> funcs;
   FuncRt *curFunc = nullptr;
@@ -1298,6 +1302,18 @@ struct osm_b200_session {
   // end of the last call's work on its stream (the next call, on whatever stream, starts behind it: the buffers are reused)
   osm::DevBuf<float> dLldRows;
   osm::CudaEvent evDevice;
+  // sinks that read a summary level and an LLD level (choose_output_level): the LLD sink's level and its parts, which the plan's union
+  // level holds next to the summary's inputs, the options of the sinks reading it, and its rows gathered out of the union rows
+  std::string lldLevel;
+  std::vector<std::string> lldLevels;
+  std::vector<std::string> lldSources;       // the levels its rows are taken from: a cVectorConcat level as the levels it joins when
+                                             // the summary's inputs hold them all, otherwise the level itself
+  CsvOpts lldCsv;
+  ArffOpts lldArff;
+  int lldParmKind = 9;
+  std::vector<int64_t> lldMeta;              // {columns, union row offsets, LLD row offsets} of the last gather, uploaded to dLldMeta
+  osm::DevBuf<int64_t> dLldMeta;
+  osm::DevBuf<float> dLldOut;                // extract_files: the gathered LLD rows
 
   // plans and functionals select their own device, the buffers above need it; a session without plans has made no CUDA call
   ~osm_b200_session() { if (device >= 0 && !plans.empty()) cudaSetDevice(device); }
@@ -1323,8 +1339,10 @@ static osm_b200_status get_plan(osm_b200_session *s, double sampleRate, int nCha
   return OSM_B200_OK;
 }
 
-// description-only plan (names, counts, frame rules) of the session's graph with `levels` as output level
-static osm_b200_status desc_plan(osm_b200_session *s, double sampleRate, int nChan, const std::vector<std::string> &levels, PlanPtr &out)
+// description-only plan (names, counts, frame rules) of the session's graph with `levels` as output level, several levels read
+// through a concat named `concat` (_unionconcat: every level keeps its own length)
+static osm_b200_status desc_plan(osm_b200_session *s, double sampleRate, int nChan, const std::vector<std::string> &levels, PlanPtr &out,
+                                 const char *concat = "_fconcat")
 {
   std::vector<osm_b200_component> cs;
   for (const osm_b200_component &c : s->comps) if (strcmp(c.name, "_sinkconcat") != 0 && strcmp(c.name, "_unionconcat") != 0) cs.push_back(c);
@@ -1337,12 +1355,12 @@ static osm_b200_status desc_plan(osm_b200_session *s, double sampleRate, int nCh
     if (levels.size() > OSM_B200_MAX_INPUTS) return hfail(OSM_B200_ERR_UNSUPPORTED, "more than 8 levels in one reader");
     osm_b200_component c;
     osm_b200_component_defaults(OSM_B200_C_VECTORCONCAT, &c);
-    snprintf(c.name, sizeof c.name, "%s", "_fconcat");
+    snprintf(c.name, sizeof c.name, "%s", concat);
     for (const std::string &l : levels) snprintf(c.reader_dmLevel[c.n_inputs++], OSM_B200_NAME_LEN, "%s", l.c_str());
-    snprintf(c.writer_dmLevel, sizeof c.writer_dmLevel, "%s", "_fconcat");
+    snprintf(c.writer_dmLevel, sizeof c.writer_dmLevel, "%s", concat);
     c.u.vectorconcat.processArrayFields = 0;
     cs.push_back(c);
-    lvl = "_fconcat";
+    lvl = concat;
   }
   osm_b200_plan *p = nullptr;
   const osm_b200_status st = osm_b200_plan_create(cs.data(), (int)cs.size(), lvl.c_str(), -1, &p);
@@ -1388,16 +1406,25 @@ static bool eval_summary(const osm_b200_session *s, const osm_b200_session::Func
   return true;
 }
 
+// the levels of the plan's output level: the summary's inputs, then the parts of the LLD sink's level not among them
+static std::vector<std::string> plan_levels(const osm_b200_session *s)
+{
+  std::vector<std::string> v = s->unionLevels;
+  for (const std::string &l : s->lldSources) if (std::find(v.begin(), v.end(), l) == v.end()) v.push_back(l);
+  return v;
+}
+
 // the functionals objects of the session for one input format; device < 0: names / counts only
 static osm_b200_status build_func_rt(osm_b200_session *s, double sampleRate, int nChan, osm_b200_plan *p, int device, osm_b200_session::FuncRt &rt)
 {
   const int K = osm_b200_plan_num_elements(p);
   // columns of every level of the plan's output level
   std::map<std::string, std::pair<int, int>> range;
-  if (s->unionLevels.size() == 1) range[s->unionLevels[0]] = {0, K};
+  const std::vector<std::string> levels = plan_levels(s);
+  if (levels.size() == 1) range[levels[0]] = {0, K};
   else {
     int o = 0;
-    for (const std::string &l : s->unionLevels) {
+    for (const std::string &l : levels) {
       PlanPtr d;
       osm_b200_status st = desc_plan(s, sampleRate, nChan, {l}, d);
       if (st != OSM_B200_OK) return st;
@@ -1408,6 +1435,23 @@ static osm_b200_status build_func_rt(osm_b200_session *s, double sampleRate, int
     if (o != K) return hfail(OSM_B200_ERR_INVALID, "cFunctionals: the levels of the summary's inputs do not add up to the plan's row");
   }
   rt.total = 0; rt.scratch = 0;
+  if (!s->lldLevels.empty()) {
+    // the LLD sink reads its levels' columns, with the row count of its own reader (the min over its levels); the summary keeps the
+    // frame counts and period of the plan it would have on its own
+    osm_b200_status st = desc_plan(s, sampleRate, nChan, s->unionLevels, rt.sum, "_unionconcat");
+    if (st == OSM_B200_OK) st = desc_plan(s, sampleRate, nChan, s->lldLevels, rt.lld);
+    if (st != OSM_B200_OK) return st;
+    for (const std::string &l : s->lldSources)
+      for (int c = 0; c < range[l].second; c++) rt.lldCols.push_back(range[l].first + c);
+    if ((int)rt.lldCols.size() != osm_b200_plan_num_elements(rt.lld.get()))
+      return hfail(OSM_B200_ERR_INVALID, "the LLD sink's levels do not add up to its row");
+    for (int k = 0; k < (int)rt.lldCols.size(); k++) {
+      rt.lldNames.push_back(osm_b200_plan_element_name(rt.lld.get(), k));
+      if (rt.lldNames.back() != osm_b200_plan_element_name(p, (int)rt.lldCols[(size_t)k]))
+        return hfail(OSM_B200_ERR_INVALID, "the LLD sink's row is not the concatenation of the levels it is taken from");
+    }
+  }
+  const osm_b200_plan *sp = rt.sum ? rt.sum.get() : p;
   for (const osm_b200_session::FuncInst &fi : s->finsts) {
     std::vector<int32_t> cols;
     std::vector<std::string> inNames;
@@ -1431,12 +1475,12 @@ static osm_b200_status build_func_rt(osm_b200_session *s, double sampleRate, int
     std::vector<const char *> names(cols.size());
     for (size_t i = 0; i < cols.size(); i++) names[i] = inNames[i].c_str();
     osm_b200_functionals *fp = nullptr;
-    osm_b200_status st = osm_b200_functionals_create(&fi.spec, (int)cols.size(), names.data(), osm_b200_plan_frame_period(p), device, &fp);
+    osm_b200_status st = osm_b200_functionals_create(&fi.spec, (int)cols.size(), names.data(), osm_b200_plan_frame_period(sp), device, &fp);
     FuncPtr f(fp);
     if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
     PlanPtr d;
-    if (plain != s->unionLevels) {
-      st = desc_plan(s, sampleRate, nChan, plain, d);
+    if (plain != s->unionLevels || rt.sum) {
+      st = desc_plan(s, sampleRate, nChan, plain, d, plain == s->unionLevels ? "_unionconcat" : "_fconcat");
       if (st != OSM_B200_OK) return st;
     }
     // preserveFields = 1 keeps the field structure of the input (functionals.cpp:133-137); for single-element fields that is the
@@ -1565,17 +1609,56 @@ static osm_b200_status read_instances(osm_b200_session *s, std::vector<const Sec
   return OSM_B200_OK;
 }
 
+static bool is_summary_level(osm_b200_session *s, const std::map<std::string, const Section *> &writerOf, const std::string &level);
+
 // pass 3: the output level: explicit, or the level the active sinks read; a multi-level sink reader is an
 // implicit concat (core/dataReader.cpp:360-444)
-static osm_b200_status choose_output_level(const char *output_level, const std::vector<std::string> &sinkLevels, std::string &lvl)
+static osm_b200_status choose_output_level(osm_b200_session *s, const char *output_level, const std::vector<std::string> &sinkLevels,
+                                           const std::map<std::string, const Section *> &writerOf)
 {
+  std::string &lvl = s->outputLevel;
   lvl = output_level ? output_level : "";
   if (!lvl.empty()) return OSM_B200_OK;
   if (sinkLevels.empty()) return hfail(OSM_B200_ERR_INVALID, "no active sink: pass output_level or enable a sink (-O / -csvoutput)");
   lvl = sinkLevels[0];
-  // every active sink gets the rows of ONE plan run: sinks that read different levels cannot be served together
-  for (const std::string &l : sinkLevels)
-    if (l != lvl) return hfail(OSM_B200_ERR_UNSUPPORTED, "the active sinks read different levels ('" + lvl + "' and '" + l + "'): enable the sinks of one level per session");
+  // every active sink gets the rows of ONE plan run.  Sinks of two levels are served together when one is a summary level and the
+  // other is not: the plan's union level then holds the LLD sink's level next to the summary's inputs
+  std::set<std::string> distinct(sinkLevels.begin(), sinkLevels.end());
+  for (const std::string &l : sinkLevels) {
+    if (l == lvl) continue;
+    const bool sumFirst = is_summary_level(s, writerOf, lvl), sumOther = is_summary_level(s, writerOf, l);
+    if (distinct.size() != 2 || sumFirst == sumOther)
+      return hfail(OSM_B200_ERR_UNSUPPORTED, "the active sinks read different levels ('" + lvl + "' and '" + l + "'): enable the sinks of one level per session");
+    s->lldLevel = sumFirst ? l : lvl;
+    lvl = sumFirst ? lvl : l;
+    break;
+  }
+  return OSM_B200_OK;
+}
+
+// the options of the sinks that read `level`, by the rules of read_instances: CSV / ARFF those of the first active sink of the
+// type (CSV: of the last cCsvSink section without one), HTK the parmKind of the last cHtkSink section
+static osm_b200_status read_level_sink_opts(const osm_b200_session *s, const std::string &level, CsvOpts &csv, ArffOpts &arff, int &parmKind)
+{
+  std::map<std::string, const Section *> secOf;
+  for (const auto &sec : s->conf.sections) if (sec.type != "cComponentManager") secOf[sec.name] = &sec;
+  bool csvLocked = false, arffLocked = false;
+  for (const auto &inst : s->conf.instances) {
+    const Section *sec = secOf.count(inst.first) ? secOf[inst.first] : nullptr;
+    const std::string *lv = sec ? sec->get("reader.dmLevel") : nullptr;
+    if (!lv || *lv != level) continue;
+    const std::string *fn = sec->get("filename");
+    const bool active = fn && *fn != "?" && !fn->empty();
+    if (inst.second == "cArffSink" && active && !arffLocked) {
+      arffLocked = true;
+      if (osm_b200_status st = read_arff_opts(*sec, arff); st != OSM_B200_OK) return st;
+    }
+    if (inst.second == "cHtkSink") { if (const std::string *pk = sec->get("parmKind")) parmKind = inum(*pk); }
+    if (inst.second == "cCsvSink" && !csvLocked) {
+      csvLocked = active;
+      if (osm_b200_status st = read_csv_opts(*sec, csv); st != OSM_B200_OK) return st;
+    }
+  }
   return OSM_B200_OK;
 }
 
@@ -1731,14 +1814,21 @@ struct SummaryBuilder {
   }
 };
 
-// pass 4 on the output level: with cFunctionals behind it, the output level becomes the union of the instances' reader levels
+// a level (or a multi-level reader's `a;b`) with cFunctionals behind it
+static bool is_summary_level(osm_b200_session *s, const std::map<std::string, const Section *> &writerOf, const std::string &level)
+{
+  const SummaryBuilder b{*s, writerOf};
+  for (const std::string &pl : split_list(level)) if (b.has_functionals(pl, 0)) return true;
+  return false;
+}
+
+// pass 4 on the output level: with cFunctionals behind it, the output level becomes the union of the instances' reader levels, and
+// of the LLD sink's levels when sinks read both
 static osm_b200_status build_summary(osm_b200_session *s, const std::map<std::string, const Section *> &writerOf)
 {
   SummaryBuilder b{*s, writerOf};
   const std::vector<std::string> parts = split_list(s->outputLevel);
-  bool anyFunc = false;
-  for (const std::string &pl : parts) anyFunc = anyFunc || b.has_functionals(pl, 0);
-  if (!anyFunc) return OSM_B200_OK;
+  if (!is_summary_level(s, writerOf, s->outputLevel)) return OSM_B200_OK;
   osm_b200_session::SummNode root;
   root.kind = 1;
   for (const std::string &pl : parts) {
@@ -1750,8 +1840,23 @@ static osm_b200_status build_summary(osm_b200_session *s, const std::map<std::st
   else { s->snodes.push_back(root); s->sroot = (int)s->snodes.size() - 1; }
   if (s->unionLevels.size() > OSM_B200_MAX_INPUTS) return hfail(OSM_B200_ERR_UNSUPPORTED, "cFunctionals: more than 8 input levels in total");
   s->hasFunc = true;
+  if (!s->lldLevel.empty()) {
+    s->lldLevels = split_list(s->lldLevel);
+    for (const std::string &l : s->lldLevels) {
+      auto it = writerOf.find(l);
+      const std::string *r = (it != writerOf.end() && it->second->type == "cVectorConcat") ? it->second->get("reader.dmLevel") : nullptr;
+      std::vector<std::string> src = r ? split_list(*r) : std::vector<std::string>();
+      bool held = !src.empty();
+      for (const std::string &x : src) held = held && std::find(s->unionLevels.begin(), s->unionLevels.end(), x) != s->unionLevels.end();
+      if (held) s->lldSources.insert(s->lldSources.end(), src.begin(), src.end());
+      else s->lldSources.push_back(l);
+    }
+    osm_b200_status st = read_level_sink_opts(s, s->outputLevel, s->csv, s->arff, s->parmKind);
+    if (st == OSM_B200_OK) st = read_level_sink_opts(s, s->lldLevel, s->lldCsv, s->lldArff, s->lldParmKind);
+    if (st != OSM_B200_OK) return st;
+  }
   s->outputLevel.clear();
-  for (const std::string &l : s->unionLevels) s->outputLevel += (s->outputLevel.empty() ? "" : ";") + l;
+  for (const std::string &l : plan_levels(s)) s->outputLevel += (s->outputLevel.empty() ? "" : ";") + l;
   return OSM_B200_OK;
 }
 
@@ -1763,6 +1868,7 @@ static osm_b200_status lower_sections(osm_b200_session *s, const std::vector<con
 {
   std::set<const Section *> need;
   std::vector<std::string> todo = split_list(s->outputLevel);
+  todo.insert(todo.end(), s->lldLevels.begin(), s->lldLevels.end());     // the LLD part's own plan description reads them
   while (!todo.empty()) {
     const std::string l = todo.back();
     todo.pop_back();
@@ -1795,7 +1901,7 @@ static osm_b200_status add_reader_concat(osm_b200_session *s)
   osm_b200_component c;
   osm_b200_component_defaults(OSM_B200_C_VECTORCONCAT, &c);
   // the union of the input levels of several cFunctionals instances keeps every level's own length (graph.cpp: padRows)
-  const char *cname = (s->hasFunc && s->unionLevels.size() > 1) ? "_unionconcat" : "_sinkconcat";
+  const char *cname = (s->hasFunc && levels.size() > 1) ? "_unionconcat" : "_sinkconcat";
   snprintf(c.name, sizeof c.name, "%s", cname);
   for (const std::string &l : levels) snprintf(c.reader_dmLevel[c.n_inputs++], OSM_B200_NAME_LEN, "%s", l.c_str());
   snprintf(c.writer_dmLevel, sizeof c.writer_dmLevel, "%s", cname);
@@ -1845,9 +1951,9 @@ try {
   std::vector<const Section *> compute;
   std::vector<std::string> sinkLevels;
   osm_b200_status st = read_instances(s.get(), compute, sinkLevels);
-  if (st == OSM_B200_OK) st = choose_output_level(output_level, sinkLevels, s->outputLevel);
   std::map<std::string, const Section *> writerOf;
   for (const Section *sec : compute) if (const std::string *w = sec->get("writer.dmLevel")) writerOf[*w] = sec;
+  if (st == OSM_B200_OK) st = choose_output_level(s.get(), output_level, sinkLevels, writerOf);
   if (st == OSM_B200_OK) st = build_summary(s.get(), writerOf);
   if (st == OSM_B200_OK) st = lower_sections(s.get(), compute, writerOf);
   if (st == OSM_B200_OK) st = add_reader_concat(s.get());
@@ -1903,6 +2009,26 @@ osm_b200_status osm_b200_session_plan(osm_b200_session *s, double sampleRate, in
 
 // a padded device batch (osm_b200_session_extract_device): its samples, stride and lengths, and the stream its work goes to
 struct DeviceBatch { const void *pcm; int64_t stride; const int64_t *lengths; cudaStream_t stream; };
+// the LLD part of a call on a session whose sinks read a summary and an LLD level: its frame offsets (n_utt + 1 entries, filled) and
+// a device buffer of at least maxRows rows for its rows (NULL: the offsets only)
+struct LldOut { int64_t *frameOff; float *dOut; int64_t maxRows; };
+
+// the LLD sink's rows out of the union rows the plan left in HBM (rows [lldOff[u], ...) of utterance u, K values each): its columns,
+// the first lo.frameOff[u + 1] - lo.frameOff[u] rows of every utterance, on `stream`
+static osm_b200_status gather_lld(osm_b200_session *s, const osm_b200_session::FuncRt &f, const float *dRows, int K, const int64_t *lldOff,
+                                  int32_t nUtt, const LldOut &lo, cudaStream_t stream)
+{
+  const size_t nc = f.lldCols.size();
+  s->lldMeta.assign(f.lldCols.begin(), f.lldCols.end());
+  s->lldMeta.insert(s->lldMeta.end(), lldOff, lldOff + nUtt);
+  s->lldMeta.insert(s->lldMeta.end(), lo.frameOff, lo.frameOff + nUtt + 1);
+  // a copy from pageable memory is staged before cudaMemcpyAsync returns; lldMeta is not touched again before the next call
+  if (s->dLldMeta.reserve(s->lldMeta.size()) != cudaSuccess ||
+      cudaMemcpyAsync(s->dLldMeta.p, s->lldMeta.data(), s->lldMeta.size() * sizeof(int64_t), cudaMemcpyHostToDevice, stream) != cudaSuccess ||
+      osm_b200_device_gather_rows(dRows, K, s->dLldMeta.p, (int32_t)nc, nUtt, lo.frameOff[nUtt], lo.dOut, stream) != 0)
+    return hfail(OSM_B200_ERR_CUDA, std::string("gather of the LLD rows: ") + cudaGetErrorString(cudaGetLastError()));
+  return OSM_B200_OK;
+}
 
 // Both extract entry points: packed PCM in host memory with `out` in host memory (dev == NULL: the plan's pipelined host run, the
 // summary on the null stream, then a copy to `out`), or a padded device batch with `out` in device memory (every launch on
@@ -1910,7 +2036,7 @@ struct DeviceBatch { const void *pcm; int64_t stride; const int64_t *lengths; cu
 // cPitchJitter flag, the cFunctionals instances' row offsets and counts).
 static osm_b200_status osm_b200_session_extract_pcm_impl(osm_b200_session *s, const void *pcm, const int64_t *uttOff, int32_t nUtt,
                                              double sampleRate, int32_t nChan, int64_t *frameOff, float *out, int64_t maxRows,
-                                             int format = OSM_B200_PCM_S16, const DeviceBatch *dev = nullptr)
+                                             int format = OSM_B200_PCM_S16, const DeviceBatch *dev = nullptr, const LldOut *lld = nullptr)
 {
   if (!s || !uttOff || !frameOff) return hfail(OSM_B200_ERR_INVALID, "null argument");
   const cudaStream_t stream = dev ? dev->stream : nullptr;
@@ -1928,6 +2054,19 @@ static osm_b200_status osm_b200_session_extract_pcm_impl(osm_b200_session *s, co
     std::vector<std::vector<int64_t>> nRows(nI, std::vector<int64_t>((size_t)nUtt));
     st = osm_b200_plan_frame_offsets(p, uttOff, nUtt, lldOff.data());
     if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
+    // the rows the summary's own plan would hold (with an LLD part the union holds more levels)
+    std::vector<int64_t> sumOff;
+    if (f->sum) {
+      sumOff.resize((size_t)nUtt + 1);
+      st = osm_b200_plan_frame_offsets(f->sum.get(), uttOff, nUtt, sumOff.data());
+      if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
+    }
+    const std::vector<int64_t> &capOff = f->sum ? sumOff : lldOff;
+    if (lld) {
+      if (!f->lld) return hfail(OSM_B200_ERR_INVALID, "the session's active sinks read one level: it has no LLD part");
+      st = osm_b200_plan_frame_offsets(f->lld.get(), uttOff, nUtt, lld->frameOff);
+      if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
+    }
     std::vector<int> live;
     frameOff[0] = 0;
     for (int u = 0; u < nUtt; u++) {
@@ -1935,16 +2074,18 @@ static osm_b200_status osm_b200_session_extract_pcm_impl(osm_b200_session *s, co
       // every instance has at least one frame
       bool all = true;
       for (size_t i = 0; i < nI; i++) {
-        const int64_t n = std::min<int64_t>(osm_b200_plan_num_frames_first_eoi(f->desc[i] ? f->desc[i].get() : p, uttOff[u + 1] - uttOff[u]), lldOff[u + 1] - lldOff[u]);
+        const int64_t n = std::min<int64_t>(osm_b200_plan_num_frames_first_eoi(f->desc[i] ? f->desc[i].get() : p, uttOff[u + 1] - uttOff[u]), capOff[u + 1] - capOff[u]);
         nRows[i][live.size()] = n;
         all = all && n > 0;
       }
       if (all) { rowOff[live.size()] = lldOff[u]; live.push_back(u); }
       frameOff[u + 1] = frameOff[u] + (all ? 1 : 0);
     }
-    if (!out) return OSM_B200_OK;
+    const int64_t nLld = lld ? lld->frameOff[nUtt] : 0;
+    if (!out && !(lld && lld->dOut)) return OSM_B200_OK;
     if (frameOff[nUtt] > maxRows) return hfail(OSM_B200_ERR_INVALID, "output buffer too small");
-    if (live.empty()) return OSM_B200_OK;
+    if (lld && (nLld > lld->maxRows || (nLld > 0 && !lld->dOut))) return hfail(OSM_B200_ERR_INVALID, "LLD output buffer too small");
+    if (live.empty() && nLld == 0) return OSM_B200_OK;
     const float *dRows = nullptr;
     if (dev) {
       if (s->dLldRows.reserve((size_t)lldOff[(size_t)nUtt] * osm_b200_plan_num_elements(p)) != cudaSuccess)
@@ -1956,6 +2097,8 @@ static osm_b200_status osm_b200_session_extract_pcm_impl(osm_b200_session *s, co
       st = osm_b200_plan_run_host_resident(p, pcm, uttOff, nUtt, lldOff.data(), &dRows);
     }
     if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
+    if (nLld > 0 && (st = gather_lld(s, *f, dRows, osm_b200_plan_num_elements(p), lldOff.data(), nUtt, *lld, stream)) != OSM_B200_OK) return st;
+    if (live.empty()) return OSM_B200_OK;
     // levels behind the SHS pitch chain: their length at the first end-of-input tick follows the Viterbi level's (data dependent)
     {
       std::vector<int32_t> lag((size_t)nUtt, -1);
@@ -1966,7 +2109,7 @@ static osm_b200_status osm_b200_session_extract_pcm_impl(osm_b200_session *s, co
         if (lag[u] < 0) continue;
         for (size_t i = 0; i < nI; i++)
           nRows[i][k] = std::max<int64_t>(0, std::min<int64_t>(osm_b200_plan_num_frames_first_eoi_v(f->desc[i] ? f->desc[i].get() : p, uttOff[u + 1] - uttOff[u], lag[u]),
-                                                               lldOff[u + 1] - lldOff[u]));
+                                                               capOff[u + 1] - capOff[u]));
       }
     }
     const int KF = f->total, KS = f->scratch;
@@ -2030,9 +2173,9 @@ osm_b200_status osm_b200_session_extract_pcm(osm_b200_session *s, const int16_t 
   catch (const std::exception &e) { return hfail(OSM_B200_ERR_INVALID, e.what()); }
 }
 
-osm_b200_status osm_b200_session_extract_device(osm_b200_session *s, const void *d_pcm, int32_t pcm_format, int64_t stride,
-                                                const int64_t *lengths, int32_t n_utt, double sample_rate, int32_t n_channels,
-                                                int64_t *frame_offsets_out, float *d_out, int64_t max_rows, void *stream)
+static osm_b200_status extract_device(osm_b200_session *s, const void *d_pcm, int32_t pcm_format, int64_t stride, const int64_t *lengths,
+                                      int32_t n_utt, double sample_rate, int32_t n_channels, int64_t *frame_offsets_out, float *d_out,
+                                      int64_t max_rows, void *stream, const LldOut *lld)
 try {
   if (!s || !lengths || !frame_offsets_out || n_utt < 0) return hfail(OSM_B200_ERR_INVALID, "null argument");
   if (pcm_format != OSM_B200_PCM_S16 && pcm_format != OSM_B200_PCM_F32)
@@ -2046,17 +2189,47 @@ try {
   }
   const DeviceBatch dev{d_pcm, stride, lengths, reinterpret_cast<cudaStream_t>(stream)};
   // the row-count query touches no device; a run starts behind the previous call's work and marks the end of its own
-  const bool run = d_out && s->device >= 0;
+  const bool run = (d_out || (lld && lld->dOut)) && s->device >= 0;
   if (run && (cudaSetDevice(s->device) != cudaSuccess || (s->evDevice && cudaStreamWaitEvent(dev.stream, s->evDevice, 0) != cudaSuccess)))
     return hfail(OSM_B200_ERR_CUDA, std::string("extract_device: ") + cudaGetErrorString(cudaGetLastError()));
   const osm_b200_status st = osm_b200_session_extract_pcm_impl(s, nullptr, uttOff.data(), n_utt, sample_rate, n_channels, frame_offsets_out,
-                                                               d_out, max_rows, pcm_format, &dev);
+                                                               d_out, max_rows, pcm_format, &dev, lld);
   if (run && ((!s->evDevice && s->evDevice.create(cudaEventDisableTiming) != cudaSuccess) || cudaEventRecord(s->evDevice, dev.stream) != cudaSuccess))
     return hfail(OSM_B200_ERR_CUDA, std::string("extract_device: ") + cudaGetErrorString(cudaGetLastError()));
   return st;
 } catch (const std::bad_alloc &) { return hfail(OSM_B200_ERR_NOMEM, "out of host memory"); }
 catch (const std::exception &e) { return hfail(OSM_B200_ERR_INVALID, e.what()); }
 
+osm_b200_status osm_b200_session_extract_device(osm_b200_session *s, const void *d_pcm, int32_t pcm_format, int64_t stride,
+                                                const int64_t *lengths, int32_t n_utt, double sample_rate, int32_t n_channels,
+                                                int64_t *frame_offsets_out, float *d_out, int64_t max_rows, void *stream)
+{
+  return extract_device(s, d_pcm, pcm_format, stride, lengths, n_utt, sample_rate, n_channels, frame_offsets_out, d_out, max_rows, stream, nullptr);
+}
+
+osm_b200_status osm_b200_session_extract_device_lld(osm_b200_session *s, const void *d_pcm, int32_t pcm_format, int64_t stride,
+                                                    const int64_t *lengths, int32_t n_utt, double sample_rate, int32_t n_channels,
+                                                    int64_t *frame_offsets_out, float *d_out, int64_t max_rows,
+                                                    int64_t *lld_frame_offsets_out, float *d_lld_out, int64_t max_lld_rows, void *stream)
+{
+  if (!lld_frame_offsets_out) return hfail(OSM_B200_ERR_INVALID, "null argument");
+  const LldOut lld{lld_frame_offsets_out, d_lld_out, max_lld_rows};
+  return extract_device(s, d_pcm, pcm_format, stride, lengths, n_utt, sample_rate, n_channels, frame_offsets_out, d_out, max_rows, stream, &lld);
+}
+
+int32_t osm_b200_session_lld_num_elements(osm_b200_session *s, double sampleRate, int32_t nChan)
+{
+  if (!s || !s->hasFunc) return 0;
+  osm_b200_plan *p;
+  osm_b200_session::FuncRt *f;
+  if (get_plan(s, sampleRate, nChan, &p) != OSM_B200_OK || get_func(s, sampleRate, nChan, p, &f) != OSM_B200_OK) return 0;
+  return (int32_t)f->lldNames.size();
+}
+
+const char *osm_b200_session_lld_element_name(osm_b200_session *s, int32_t idx)
+{
+  return (s && s->curFunc && idx >= 0 && (size_t)idx < s->curFunc->lldNames.size()) ? s->curFunc->lldNames[(size_t)idx].c_str() : nullptr;
+}
 
 osm_b200_status osm_b200_session_extract_files(osm_b200_session *s, int32_t n, const char *const *wavPaths,
                                                const char *const *htkPaths, const char *const *csvPaths, int64_t *framesOut)
@@ -2093,8 +2266,11 @@ static bool parallel_files(int n, Fn fn, std::string &err, bool serial = false)
   return !failed.load();
 }
 
+// the options of the sinks of one level, and the plan whose row times their time stamps are
+struct SinkOpts { const CsvOpts &csv; const ArffOpts &arff; int parmKind; const osm_b200_plan *timePlan; };
+
 // the sinks of one batch: rows [fo[k], fo[k+1]) of file idx[k] -> its HTK / CSV / ARFF files, files in parallel
-static bool write_batch(osm_b200_session *s, const std::vector<int> &idx, const int64_t *fo, const int64_t *nTime, const float *rows, int K,
+static bool write_batch(const SinkOpts &o, const std::vector<int> &idx, const int64_t *fo, const int64_t *nTime, const float *rows, int K,
                         const std::vector<std::string> &names, double period, const char *const *htkPaths, const char *const *csvPaths,
                         const char *const *arffPaths, int64_t *framesOut, std::string &err, const DevText *dt = nullptr,
                         const uint32_t *packed = nullptr, const DevText *dtArff = nullptr)
@@ -2114,24 +2290,44 @@ static bool write_batch(osm_b200_session *s, const std::vector<int> &idx, const 
     const float *r = rows + (size_t)fo[k] * K;
     const int64_t nr = fo[k + 1] - fo[k];
     if (framesOut) framesOut[i] = nr;
-    if (htkPaths && htkPaths[i] && !write_htk(htkPaths[i], r, nr, K, period, s->parmKind, e, packed ? packed + (size_t)fo[k] * K : nullptr)) return false;
+    if (htkPaths && htkPaths[i] && !write_htk(htkPaths[i], r, nr, K, period, o.parmKind, e, packed ? packed + (size_t)fo[k] * K : nullptr)) return false;
     DevText dk;
     if (dt) dk = DevText{dt->text + fo[k] * dt->slot, dt->slot, dt->len + fo[k], dt->host + fo[k]};
-    if (csvPaths && csvPaths[i] && !write_csv(csvPaths[i], r, nr, K, names, period, s->csv, e, nTime[k], dt ? &dk : nullptr, s->cur)) return false;
+    if (csvPaths && csvPaths[i] && !write_csv(csvPaths[i], r, nr, K, names, period, o.csv, e, nTime[k], dt ? &dk : nullptr, o.timePlan)) return false;
     DevText da;
     if (dtArff) da = DevText{dtArff->text + fo[k] * dtArff->slot, dtArff->slot, dtArff->len + fo[k], dtArff->host + fo[k]};
-    if (arffPaths && arffPaths[i] && !write_arff(arffPaths[i], r, nr, K, names, period, s->arff, e, nTime[k], dtArff ? &da : nullptr, s->cur)) return false;
+    if (arffPaths && arffPaths[i] && !write_arff(arffPaths[i], r, nr, K, names, period, o.arff, e, nTime[k], dtArff ? &da : nullptr, o.timePlan)) return false;
     return true;
   }, err, shared);
 }
 }  // extern "C++"
 
-// no exception crosses the C boundary (allocation failures on hostile inputs, std::filesystem / stream errors)
 osm_b200_status osm_b200_session_extract_files_arff(osm_b200_session *s, int32_t n, const char *const *wavPaths,
                                                     const char *const *htkPaths, const char *const *csvPaths,
                                                     const char *const *arffPaths, int64_t *framesOut)
+{
+  return osm_b200_session_extract_files_lld(s, n, wavPaths, htkPaths, csvPaths, arffPaths, nullptr, nullptr, nullptr, framesOut);
+}
+
+// the rows [n][K] of one level in HBM -> their CSV / ARFF value text and HTK payload, formatted on the device, and the rows themselves
+// in host memory; false on a CUDA error
+static bool device_sink_rows(const float *dRows, int64_t n, int K, bool wantCsv, char csvDelim, bool wantArff, bool wantHtk,
+                             std::vector<float> &rows, HostText &csv, HostText &arff, std::vector<uint32_t> &packed)
+{
+  return cudaMemcpy(rows.data(), dRows, (size_t)n * K * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess &&
+         (!wantCsv || device_text(dRows, n, K, csvDelim, false, csv)) &&
+         (!wantArff || device_text(dRows, n, K, ',', true, arff)) && (!wantHtk || device_htk(dRows, n, K, packed));
+}
+
+// no exception crosses the C boundary (allocation failures on hostile inputs, std::filesystem / stream errors)
+osm_b200_status osm_b200_session_extract_files_lld(osm_b200_session *s, int32_t n, const char *const *wavPaths,
+                                                   const char *const *htkPaths, const char *const *csvPaths, const char *const *arffPaths,
+                                                   const char *const *lldHtkPaths, const char *const *lldCsvPaths,
+                                                   const char *const *lldArffPaths, int64_t *framesOut)
 try {
   if (!s || !wavPaths || n < 0) return hfail(OSM_B200_ERR_INVALID, "null argument");
+  const bool wantLld = lldHtkPaths || lldCsvPaths || lldArffPaths;
+  if (wantLld && s->lldLevel.empty()) return hfail(OSM_B200_ERR_INVALID, "LLD paths given, but the session's active sinks read one level: it has no LLD part");
   if (osm_b200_status st = after_device_calls(s); st != OSM_B200_OK) return st;
   // files of one call are grouped by (sample rate, channels); each group is one batched plan run
   std::vector<Wav> wavs(n);
@@ -2142,7 +2338,7 @@ try {
   bool sharedAcross = false;
   {
     std::map<std::string, std::pair<int, int>> owner;                 // path -> (rate, channels/format) of its first writer
-    for (const char *const *paths : {htkPaths, csvPaths, arffPaths})
+    for (const char *const *paths : {htkPaths, csvPaths, arffPaths, lldHtkPaths, lldCsvPaths, lldArffPaths})
       if (paths)
         for (int i = 0; i < n; i++) {
           if (!paths[i]) continue;
@@ -2189,9 +2385,37 @@ try {
       K = f->total;
       names = f->names;
       rows.resize((size_t)nG * K + 1);
-      st = osm_b200_session_extract_pcm_impl(s, pcm.data(), off.data(), nG, sr, nc, fo.data(), rows.data(), nG, fmt);
+      // the LLD sink's rows of the same plan run: gathered on the device, formatted there as for an LLD-only session, and written by
+      // write_batch with the options of the sinks that read its level
+      std::vector<int64_t> lfo(wantLld ? (size_t)nG + 1 : 0), lTime(wantLld ? (size_t)nG : 0);
+      LldOut lo{lfo.data(), nullptr, 0};
+      if (wantLld) {
+        st = osm_b200_plan_frame_offsets(f->lld.get(), off.data(), nG, lfo.data());
+        if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
+        lo.maxRows = lfo[(size_t)nG];
+        if (s->dLldOut.reserve((size_t)lo.maxRows * f->lldCols.size() + 1) != cudaSuccess) return hfail(OSM_B200_ERR_NOMEM, "out of device memory (LLD rows)");
+        lo.dOut = s->dLldOut.p;
+      }
+      st = osm_b200_session_extract_pcm_impl(s, pcm.data(), off.data(), nG, sr, nc, fo.data(), rows.data(), nG, fmt, nullptr, wantLld ? &lo : nullptr);
       if (st != OSM_B200_OK) return st;
       for (int k = 0; k < nG; k++) nTime[k] = fo[k + 1] - fo[k];
+      if (wantLld) {
+        const int KL = (int)f->lldCols.size();
+        const int64_t nR = lfo[(size_t)nG];
+        std::vector<float> lrows((size_t)nR * KL + 1);
+        HostText lcsv, larff;
+        std::vector<uint32_t> lpacked;
+        const bool lText = devSinks && nR > 0;
+        if (nR > 0 && !(lText ? device_sink_rows(s->dLldOut.p, nR, KL, lldCsvPaths, s->lldCsv.delim, lldArffPaths, lldHtkPaths, lrows, lcsv, larff, lpacked)
+                              : cudaMemcpy(lrows.data(), s->dLldOut.p, (size_t)nR * KL * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess))
+          return hfail(OSM_B200_ERR_CUDA, std::string("device sinks: ") + cudaGetErrorString(cudaGetLastError()));
+        for (int k = 0; k < nG; k++) lTime[k] = osm_b200_plan_num_time_frames(f->lld.get(), off[k + 1] - off[k]);
+        const DevText dt = lcsv.view(), dtA = larff.view();
+        if (!write_batch(SinkOpts{s->lldCsv, s->lldArff, s->lldParmKind, f->lld.get()}, g.second, lfo.data(), lTime.data(), lrows.data(), KL, f->lldNames,
+                         osm_b200_plan_frame_period(f->lld.get()), lldHtkPaths, lldCsvPaths, lldArffPaths, nullptr, err, lText && lldCsvPaths ? &dt : nullptr,
+                         lText && lldHtkPaths ? lpacked.data() : nullptr, lText && lldArffPaths ? &dtA : nullptr))
+          return hfail(OSM_B200_ERR_INVALID, err);
+      }
     } else {
       st = osm_b200_plan_frame_offsets(p, off.data(), nG, fo.data());
       if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
@@ -2206,17 +2430,16 @@ try {
         const float *dRows = nullptr;
         st = osm_b200_plan_run_host_resident(p, pcm.data(), off.data(), nG, fo.data(), &dRows);
         if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
-        const bool ok = cudaMemcpy(rows.data(), dRows, (size_t)nR * K * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess &&
-                        (!wantCsv || device_text(dRows, nR, K, s->csv.delim, false, csv)) &&
-                        (!wantArff || device_text(dRows, nR, K, ',', true, arff)) && (!wantHtk || device_htk(dRows, nR, K, packed));
-        if (!ok) return hfail(OSM_B200_ERR_CUDA, std::string("device sinks: ") + cudaGetErrorString(cudaGetLastError()));
+        if (!device_sink_rows(dRows, nR, K, wantCsv, s->csv.delim, wantArff, wantHtk, rows, csv, arff, packed))
+          return hfail(OSM_B200_ERR_CUDA, std::string("device sinks: ") + cudaGetErrorString(cudaGetLastError()));
       } else {
         st = osm_b200_plan_run_host(p, pcm.data(), off.data(), nG, fo.data(), rows.data());
         if (st != OSM_B200_OK) return hfail(st, osm_b200_last_error());
       }
     }
     const DevText dt = csv.view(), dtA = arff.view();
-    if (!write_batch(s, g.second, fo.data(), nTime.data(), rows.data(), K, names, osm_b200_plan_frame_period(p), htkPaths, csvPaths, arffPaths, framesOut, err,
+    const double period = s->hasFunc ? osm_b200_plan_frame_period(s->curFunc->sum ? s->curFunc->sum.get() : p) : osm_b200_plan_frame_period(p);
+    if (!write_batch(SinkOpts{s->csv, s->arff, s->parmKind, s->cur}, g.second, fo.data(), nTime.data(), rows.data(), K, names, period, htkPaths, csvPaths, arffPaths, framesOut, err,
                      devText && wantCsv ? &dt : nullptr, devText && wantHtk ? packed.data() : nullptr, devText && wantArff ? &dtA : nullptr))
       return hfail(OSM_B200_ERR_INVALID, err);
   }
@@ -2251,7 +2474,8 @@ osm_b200_status osm_b200_session_write_files(osm_b200_session *s, double sampleR
     for (int i = 0; i < n; i++) nTime[i] = frameOff[i + 1] - frameOff[i];
   }
   std::string err;
-  if (!write_batch(s, idx, frameOff, nTime.data(), rows, K, names, osm_b200_plan_frame_period(p), htkPaths, csvPaths, arffPaths, nullptr, err))
+  if (!write_batch(SinkOpts{s->csv, s->arff, s->parmKind, s->cur}, idx, frameOff, nTime.data(), rows, K, names, osm_b200_plan_frame_period(p), htkPaths,
+                   csvPaths, arffPaths, nullptr, err))
     return hfail(OSM_B200_ERR_INVALID, err);
   return OSM_B200_OK;
 }

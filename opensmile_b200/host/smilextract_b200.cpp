@@ -3,6 +3,8 @@
 // 42-174): -C config, -I input.wav, plus every option the config declares through \cm[...]
 // (-O / -output htk, -csvoutput csv, -instname name, ...).  Batch mode: -I may be given several
 // times (or -filelist F with one "wav[ htk[ csv]]" per line); all files go through ONE plan run.
+// When the active sinks read a summary level and an LLD level (-csvoutput with -lldcsvoutput of the shipped feature
+// sets), that one run writes both: -O / -output / -csvoutput name the summary's files, -lld*output the LLD sinks' files.
 #include <cstdio>
 #include <cstring>
 #include <fstream>
@@ -23,6 +25,7 @@ int main(int argc, char **argv)
   std::string conf, level;
   std::vector<std::string> wavs, htks, csvs, arffs, optN, optV;
   std::string outHtk, outCsv, outArff, htkDir, csvDir;
+  std::string sumHtk, sumCsv, lldHtk, lldCsv;             // the same options apart, for a session with an LLD part
   int device = 0;
   for (int i = 1; i < argc; i++) {
     const std::string a = argv[i];
@@ -63,6 +66,10 @@ int main(int argc, char **argv)
       if (n == "O" || n == "output" || n == "lldhtkoutput") outHtk = v;
       if (n == "csvoutput" || n == "lldcsvoutput") outCsv = v;
       if (n == "lldarffoutput") outArff = v;
+      if (n == "O" || n == "output") sumHtk = v;
+      if (n == "csvoutput") sumCsv = v;
+      if (n == "lldhtkoutput") lldHtk = v;
+      if (n == "lldcsvoutput") lldCsv = v;
     }
   }
   if (conf.empty() || wavs.empty()) { fprintf(stderr, "SMILExtract_b200: -C <config> and -I <wav> are required (-h for help)\n"); return 2; }
@@ -89,7 +96,25 @@ int main(int argc, char **argv)
     return 1;
   }
   std::vector<int64_t> frames(wavs.size(), 0);
-  const osm_b200_status st = osm_b200_session_extract_files_arff(s, (int)wavs.size(), pw.data(), ph.data(), pc.data(), pa.data(), frames.data());
+  // the LLD part exists for every input format or for none (16 kHz mono asks the session which)
+  const bool both = osm_b200_session_lld_num_elements(s, 16000.0, 1) > 0;
+  std::vector<std::string> lh(wavs.size()), lc(wavs.size());
+  std::vector<const char *> plh, plc;
+  for (size_t k = 0; k < wavs.size() && both; k++) {
+    // -filelist names the summary's files; several inputs get the LLD files <input>.lld.htk / .lld.csv
+    if (!outHtk.empty()) htks[k] = sumHtk.empty() ? std::string() : (wavs.size() == 1 ? sumHtk : replace_ext(wavs[k], ".htk"));
+    if (!outCsv.empty()) csvs[k] = sumCsv.empty() ? std::string() : (wavs.size() == 1 ? sumCsv : replace_ext(wavs[k], ".csv"));
+    if (!lldHtk.empty()) lh[k] = wavs.size() == 1 ? lldHtk : replace_ext(wavs[k], ".lld.htk");
+    if (!lldCsv.empty()) lc[k] = wavs.size() == 1 ? lldCsv : replace_ext(wavs[k], ".lld.csv");
+    ph[k] = htks[k].empty() ? nullptr : htks[k].c_str();
+    pc[k] = csvs[k].empty() ? nullptr : csvs[k].c_str();
+    plh.push_back(lh[k].empty() ? nullptr : lh[k].c_str());
+    plc.push_back(lc[k].empty() ? nullptr : lc[k].c_str());
+  }
+  const osm_b200_status st = both ? osm_b200_session_extract_files_lld(s, (int)wavs.size(), pw.data(), ph.data(), pc.data(), nullptr,
+                                                                       lldHtk.empty() ? nullptr : plh.data(), lldCsv.empty() ? nullptr : plc.data(),
+                                                                       outArff.empty() ? nullptr : pa.data(), frames.data())
+                                  : osm_b200_session_extract_files_arff(s, (int)wavs.size(), pw.data(), ph.data(), pc.data(), pa.data(), frames.data());
   if (st != OSM_B200_OK) { fprintf(stderr, "SMILExtract_b200: %s\n", osm_b200_host_last_error()); osm_b200_session_close(s); return 1; }
   for (size_t k = 0; k < wavs.size(); k++) fprintf(stderr, "%s: %ld frames\n", wavs[k].c_str(), (long)frames[k]);
   osm_b200_session_close(s);

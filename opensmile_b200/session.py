@@ -55,6 +55,11 @@ class Session:
             raise SessionError(capi.ERR_INVALID, self._L.osm_b200_host_last_error().decode())
         return [self._L.osm_b200_session_element_name(self._h, i).decode() for i in range(n)]
 
+    def lld_element_names(self, sample_rate=16000.0, n_channels=1):
+        """names of the LLD part of a session whose sinks read a summary and an LLD level ([] without one)"""
+        n = self._L.osm_b200_session_lld_num_elements(self._h, float(sample_rate), n_channels)
+        return [self._L.osm_b200_session_lld_element_name(self._h, i).decode() for i in range(n)]
+
     def components(self, sample_rate=16000.0, n_channels=1):
         """the osm_b200_component list the config resolved to, and the output level"""
         p = C.POINTER(capi.Component)()
@@ -87,7 +92,7 @@ class Session:
             fo.ctypes.data_as(i64p), out.ctypes.data, out.shape[0]))
         return out, fo
 
-    def extract_tensor(self, pcm, lengths, sample_rate):
+    def extract_tensor(self, pcm, lengths, sample_rate, with_lld=False):
         """Audio already on the GPU -> (rows, frame_offsets), the pair extract_pcm returns, without a host round trip.
 
         pcm: a contiguous CUDA tensor on the session's device, int16 or float32, shaped [B, L] (mono) or [B, C, L]
@@ -97,7 +102,9 @@ class Session:
         smilePcm_convertFloatSamples).  Channels are mixed down as for a WAV file.
         lengths: B sample-frame counts, a host sequence or a CPU tensor.
         The work is enqueued on torch.cuda.current_stream(pcm.device).  rows: a CUDA float32 tensor
-        [frame_offsets[-1], num_elements] on pcm's device; frame_offsets: a numpy int64 array of B + 1 entries."""
+        [frame_offsets[-1], num_elements] on pcm's device; frame_offsets: a numpy int64 array of B + 1 entries.
+        with_lld=True, on a session whose sinks read a summary and an LLD level: (rows, frame_offsets, lld_rows, lld_frame_offsets),
+        the summary and the LLD sinks' rows of one plan run, as the two single-level sessions give them."""
         import torch
         if not isinstance(pcm, torch.Tensor):
             raise TypeError("pcm must be a torch tensor")
@@ -125,19 +132,30 @@ class Session:
         i64p = C.POINTER(C.c_int64)
         stream = C.c_void_p(torch.cuda.current_stream(pcm.device).cuda_stream)
         fo = np.zeros(n_utt + 1, dtype=np.int64)
+        lfo = np.zeros(n_utt + 1, dtype=np.int64)
 
-        def call(d_out, max_rows):
-            self._check(self._L.osm_b200_session_extract_device(
-                self._h, C.c_void_p(pcm.data_ptr()), fmt, stride, lens.ctypes.data_as(i64p), n_utt, float(sample_rate), n_chan,
-                fo.ctypes.data_as(i64p), d_out, max_rows, stream))
+        def call(d_out, max_rows, d_lld=None, max_lld=0):
+            args = (self._h, C.c_void_p(pcm.data_ptr()), fmt, stride, lens.ctypes.data_as(i64p), n_utt, float(sample_rate), n_chan,
+                    fo.ctypes.data_as(i64p), d_out, max_rows)
+            if with_lld:
+                self._check(self._L.osm_b200_session_extract_device_lld(*args, lfo.ctypes.data_as(i64p), d_lld, max_lld, stream))
+            else:
+                self._check(self._L.osm_b200_session_extract_device(*args, stream))
         call(None, 0)
         n_el = self._L.osm_b200_session_num_elements(self._h, float(sample_rate), n_chan)
         if n_el <= 0:
             raise SessionError(capi.ERR_INVALID, self._L.osm_b200_host_last_error().decode())
         rows = torch.empty((int(fo[-1]), n_el), dtype=torch.float32, device=pcm.device)
-        if rows.numel():
-            call(C.c_void_p(rows.data_ptr()), rows.shape[0])
-        return rows, fo
+        if not with_lld:
+            if rows.numel():
+                call(C.c_void_p(rows.data_ptr()), rows.shape[0])
+            return rows, fo
+        n_lld = self._L.osm_b200_session_lld_num_elements(self._h, float(sample_rate), n_chan)
+        lld = torch.empty((int(lfo[-1]), n_lld), dtype=torch.float32, device=pcm.device)
+        if rows.numel() or lld.numel():
+            call(C.c_void_p(rows.data_ptr() if rows.numel() else None), rows.shape[0],
+                 C.c_void_p(lld.data_ptr() if lld.numel() else None), lld.shape[0])
+        return rows, fo, lld, lfo
 
     def sink_options(self):
         """formatting options of the configuration's active sinks, as text (osm_b200_session_sink_options)"""
@@ -157,13 +175,19 @@ class Session:
             ns.ctypes.data_as(i64p) if ns is not None else None, rows.ctypes.data,
             _strs(htk_paths) if htk_paths else None, _strs(csv_paths) if csv_paths else None, _strs(arff_paths) if arff_paths else None))
 
-    def extract_files(self, wav_paths, htk_paths=None, csv_paths=None, arff_paths=None):
+    def extract_files(self, wav_paths, htk_paths=None, csv_paths=None, arff_paths=None,
+                      lld_htk_paths=None, lld_csv_paths=None, lld_arff_paths=None):
+        """lld_*_paths: the LLD sinks' files of a session whose sinks read a summary and an LLD level, from the same plan run"""
         n = len(wav_paths)
         frames = np.zeros(n, dtype=np.int64)
-        self._check(self._L.osm_b200_session_extract_files_arff(
-            self._h, n, _strs(wav_paths), _strs(htk_paths) if htk_paths else None,
-            _strs(csv_paths) if csv_paths else None, _strs(arff_paths) if arff_paths else None,
-            frames.ctypes.data_as(C.POINTER(C.c_int64))))
+        paths = [_strs(p) if p else None for p in (htk_paths, csv_paths, arff_paths)]
+        if lld_htk_paths or lld_csv_paths or lld_arff_paths:
+            lld = [_strs(p) if p else None for p in (lld_htk_paths, lld_csv_paths, lld_arff_paths)]
+            self._check(self._L.osm_b200_session_extract_files_lld(
+                self._h, n, _strs(wav_paths), *paths, *lld, frames.ctypes.data_as(C.POINTER(C.c_int64))))
+        else:
+            self._check(self._L.osm_b200_session_extract_files_arff(
+                self._h, n, _strs(wav_paths), *paths, frames.ctypes.data_as(C.POINTER(C.c_int64))))
         return frames
 
 
