@@ -584,6 +584,11 @@ OSM_B200_API osm_b200_status osm_b200_plan_profile_entry(osm_b200_plan *plan, in
  * Any pointer may be NULL. */
 OSM_B200_API osm_b200_status osm_b200_plan_last_lld_launch(const osm_b200_plan *plan, const char **kernel, int32_t *grid,
                                                            int64_t *n_chunks);
+/* The last run_* call: *pieces = pipeline pieces run_host cut the batch into (0 for run_device), *spectral_staged = 1 when the
+ * last spectral_kernel launch staged its magnitude tile in shared memory, 0 when it read it from global memory, -1 when the run
+ * launched none; *spectral_smem = that launch's dynamic shared memory in bytes.  Any pointer may be NULL. */
+OSM_B200_API osm_b200_status osm_b200_plan_last_run_info(const osm_b200_plan *plan, int32_t *pieces, int32_t *spectral_staged,
+                                                         int32_t *spectral_smem);
 
 #ifdef __cplusplus
 }

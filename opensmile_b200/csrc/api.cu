@@ -241,6 +241,8 @@ struct osm_b200_plan {
   std::vector<const char *> profName;
   int profN = 0;
   LldLaunchInfo lastInfo{};
+  // osm_b200_plan_last_run_info: pipeline pieces of the last run, the last spectral_kernel launch's staging path and shared memory
+  int lastPieces = 0, lastSpecStaged = -1, lastSpecSmem = 0;
 
   // work still in flight may use any member: drain the device before they release themselves
   ~osm_b200_plan()
@@ -1361,7 +1363,7 @@ static osm_b200_status launch_range(osm_b200_plan *pl, const void *d_pcm, float 
       sp.mag = rt.dMag.p + (size_t)t0 * sp.nSrc * sp.F;
       sp.tiles = rt.dTiles.p + t0; sp.nTiles = t1 - t0;
       sp.statOff = dS; sp.stat = pl->dStat.p;
-      CU(launch_spectral(sp, st));
+      CU(launch_spectral(sp, st, &pl->lastSpecStaged, &pl->lastSpecSmem));
       PROF("spectral_kernel");
     } else if (o.kind == SOP_PITCH) {
       ShsParams sh = o.shs;
@@ -1513,6 +1515,7 @@ static osm_b200_status run_device_impl(osm_b200_plan *pl, const void *d_pcm, con
   CU(cudaSetDevice(pl->device));
   pl->lastLaunches = 0;
   pl->lastInfo = LldLaunchInfo{};
+  pl->lastPieces = 0; pl->lastSpecStaged = -1; pl->lastSpecSmem = 0;
   pl->timed = false;
   pl->profN = 0;
   osm_b200_status s = prepare_batch(pl, utt_offsets, n_utt, frame_offsets, st);
@@ -1578,6 +1581,7 @@ static osm_b200_status run_host_impl(osm_b200_plan *pl, const void *pcm, const i
   cudaStream_t st = pl->hostStream;
   pl->lastLaunches = 0;
   pl->lastInfo = LldLaunchInfo{};
+  pl->lastPieces = 0; pl->lastSpecStaged = -1; pl->lastSpecSmem = 0;
   pl->timed = false;
   osm_b200_status s = prepare_batch(pl, utt_offsets, n_utt, frame_offsets, st);
   if (s != OSM_B200_OK) return s;
@@ -1623,6 +1627,7 @@ static osm_b200_status run_host_impl(osm_b200_plan *pl, const void *pcm, const i
       cudaStreamSynchronize(pl->h2dStream); cudaStreamSynchronize(st); cudaStreamSynchronize(pl->d2hStream);
       return s;
     }
+    pl->lastPieces++;
     CU(cudaEventRecord(pl->evPiece[2 * k + 1], st));
     CU(cudaStreamWaitEvent(pl->d2hStream, pl->evPiece[2 * k + 1], 0));
     const long long ra = hR[u0], rb = hR[u1];
@@ -1738,6 +1743,15 @@ osm_b200_status osm_b200_plan_last_lld_launch(const osm_b200_plan *pl, const cha
   if (kernel) *kernel = pl->lastInfo.kernel;
   if (grid) *grid = pl->lastInfo.grid;
   if (n_chunks) *n_chunks = pl->lastInfo.nChunks;
+  return OSM_B200_OK;
+}
+
+osm_b200_status osm_b200_plan_last_run_info(const osm_b200_plan *pl, int32_t *pieces, int32_t *spectral_staged, int32_t *spectral_smem)
+{
+  if (!pl) return fail(OSM_B200_ERR_INVALID, "null plan");
+  if (pieces) *pieces = pl->lastPieces;
+  if (spectral_staged) *spectral_staged = pl->lastSpecStaged;
+  if (spectral_smem) *spectral_smem = pl->lastSpecSmem;
   return OSM_B200_OK;
 }
 

@@ -629,6 +629,16 @@ struct GraphCompiler {
     po.maxPitch = pp.maxPitch < 0.0 ? 0.0 : pp.maxPitch;                       // lldcore/pitchACF.cpp:101-102
     po.voicingCutoff = pp.voicingCutoff > 1.0 ? 1.0 : (pp.voicingCutoff < 0.0 ? 0.0 : pp.voicingCutoff);
     po.fsSec = (float)fe.fftFrameSizeSec;                                       // :107-110
+    // preskip = 1 / (maxPitch * Tsamp) lags (:155-159) indexes the concatenated [acf ; cepstrum] input of 2 * (nfft / 2)
+    // elements; from preskip = nfft on, the reference reads past it
+    const int preskip = po.maxPitch <= 0.0 ? 0 : (int)(1.0 / (po.maxPitch * ((double)po.fsSec / (double)fe.nfft)));
+    if (preskip >= fe.nfft) {
+      char buf[512];
+      snprintf(buf, sizeof buf, "cPitchACF: maxPitch = %g Hz skips %d lags, not fewer than the %d elements of [acf ; cepstrum]",
+               po.maxPitch, preskip, fe.nfft);
+      err = buf;
+      return OSM_B200_ERR_UNSUPPORTED;
+    }
     po.voiceProb = pp.voiceProb != 0; po.voiceQual = pp.voiceQual != 0; po.HNR = pp.HNR != 0; po.HNRdB = pp.HNRdB != 0;
     po.linHNR = pp.linHNR != 0; po.F0 = pp.F0 != 0; po.F0raw = pp.F0raw != 0; po.F0env = pp.F0env != 0;
     const std::pair<bool, const char *> outputs[] = {                           // :112-121

@@ -293,7 +293,9 @@ __global__ void __launch_bounds__(NT, 1) acf_pitch_kernel(const AcfPitchParams p
     sCmax[vw * F + f] = cmax; sCsum[vw * F + f] = csum;
   }
   __syncthreads();
-  double mean = acf(preskip), mx = acf(n - 1), cmax = cep(n - 1), csum = 0.0;
+  // the reference starts the mean with element preskip of the concatenated input [acf ; cepstrum] (:258): past the ACF's n
+  // lags that is a cepstrum value.  The plan refuses preskip >= 2n, where the reference reads outside its input
+  double mean = preskip < n ? acf(preskip) : cep(preskip - n), mx = acf(n - 1), cmax = cep(n - 1), csum = 0.0;
   int zcr = 0;
   for (int w = 0; w < NVW; w++) {
     zcr += sZcr[w * F + f];

@@ -225,7 +225,8 @@ cudaError_t launch_cms_means(const PostParams &p, float *means, int u0, int u1, 
 cudaError_t launch_vecop_ll1(float *stat, int statStride, int srcCol, int n, int outCol, long long row0, long long row1,
                              cudaStream_t st);
 
-cudaError_t launch_spectral(const SpectralParams &p, cudaStream_t st);
+// *staged (optional): 1 when the magnitude tile was staged in shared memory; *smem (optional): dynamic shared memory of the launch
+cudaError_t launch_spectral(const SpectralParams &p, cudaStream_t st, int *staged = nullptr, int *smemBytes = nullptr);
 // cFFTmagphase as an output level: tile-major magnitude level [tile][nSrc][F] -> columns of the static rows
 cudaError_t launch_mag_rows(const float *mag, const OpTile *tiles, int nTiles, int F, int nSrc, const long long *statOff,
                             float *stat, int statStride, int outCol, cudaStream_t st, int mode = 0, float fftN = 1.f, float dBpnorm = 0.f,

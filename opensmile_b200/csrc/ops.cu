@@ -17,8 +17,8 @@ constexpr int kSpecThreads = 32 * kSpecWarps;   // one CTA = one tile; lane = fr
 struct SpecView {
   const float *mag;     // magnitudes of this frame: bin k at mag[k * mstride] (shared-memory tile, stride 32,
                         // or -- when both tiles do not fit -- the global tile, stride F)
-  const float *logS;    // shared-memory log spectrum of this frame, bin k at logS[k * 32] (or null)
-  int mstride;
+  const float *logS;    // shared-memory log spectrum of this frame, bin k at logS[k * lstride] (or null)
+  int mstride, lstride;
   int squareInput, useLog;
   __device__ __forceinline__ float m(int k) const { return mag[(size_t)k * mstride]; }
   __device__ __forceinline__ float M(int k) const   // srcM (:677-690)
@@ -31,7 +31,7 @@ struct SpecView {
     const float v = m(k);
     return squareInput ? __fmul_rn(v, v) : v;
   }
-  __device__ __forceinline__ float L(int k) const { return logS[k * 32]; }
+  __device__ __forceinline__ float L(int k) const { return logS[k * lstride]; }
   __device__ __forceinline__ float LP(int k) const { return useLog ? L(k) : P(k); }
 };
 
@@ -42,7 +42,7 @@ struct SpecView {
 // same loop, so the split does not change any result.
 __global__ void __launch_bounds__(kSpecThreads) spectral_kernel(const SpectralParams p)
 {
-  extern __shared__ float ssm[];       // [nSrc][32] magnitudes | [nSrc][32] log spectrum (when reqLog) | [32] previous frame's column is read from global
+  extern __shared__ float ssm[];       // [nSrc][32] magnitudes (when staged) | [nSrc][F] log spectrum (when reqLog); the previous frame's column is read from global
   const OpTile tl = p.tiles[blockIdx.x];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const bool active = lane < tl.nf;
@@ -62,6 +62,7 @@ __global__ void __launch_bounds__(kSpecThreads) spectral_kernel(const SpectralPa
   v.mag = staged ? (smag + fl) : (gmag + fl);
   v.mstride = staged ? 32 : F;
   v.logS = slog + fl;
+  v.lstride = F;
   v.squareInput = p.squareInput; v.useLog = p.useLog;
   const double F0 = p.F0;
   const int lo = p.loBin, hi = p.hiBin, nBins = hi - lo + 1;
@@ -73,11 +74,12 @@ __global__ void __launch_bounds__(kSpecThreads) spectral_kernel(const SpectralPa
     if (p.reqPow) src = 0;
     else if (p.reqMag) src = 1;
     else src = 2;
-    SpecView vl = v;     // inactive lanes compute the shadow column too: every slog column is defined
-    for (int k = warp; k < Nsrc; k += kSpecWarps) {
-      const float x = (src == 0) ? vl.P(k) : ((src == 1) ? vl.M(k) : vl.m(k));
-      slog[k * 32 + lane] = (x <= specFloor) ? p.logSpecFloor : __fmul_rn(fac, logf(x));
-    }
+    // one column per frame of the tile (F of them): lanes beyond F shadow frame 0 and read column 0, which lane 0 writes
+    if (lane < F)
+      for (int k = warp; k < Nsrc; k += kSpecWarps) {
+        const float x = (src == 0) ? v.P(k) : ((src == 1) ? v.M(k) : v.m(k));
+        slog[k * F + lane] = (x <= specFloor) ? p.logSpecFloor : __fmul_rn(fac, logf(x));
+      }
     __syncthreads();
   }
 
@@ -326,16 +328,19 @@ __global__ void __launch_bounds__(kSpecThreads) spectral_kernel(const SpectralPa
   }
 }
 
-cudaError_t launch_spectral(const SpectralParams &p, cudaStream_t st)
+cudaError_t launch_spectral(const SpectralParams &p, cudaStream_t st, int *staged, int *smemBytes)
 {
   if (p.nTiles <= 0) return cudaSuccess;
   // Stage the magnitude tile in shared memory only together with a log spectrum (measured: without
   // one, the extra shared memory costs more occupancy than the cached global reads cost time), and
-  // only when both tiles fit (they do up to FFT 1024)
+  // only when both tiles fit (they do up to FFT 1024).  The log spectrum holds one column per frame
+  // of the tile: F = 8 at FFT 4096 keeps it at 64 KB, where 32 columns would pass the opt-in limit.
   const size_t tile = (size_t)p.nSrc * 32 * sizeof(float);
   SpectralParams q = p;
   q.stageMag = (p.reqLog && tile * 2 <= 200 * 1024) ? 1 : 0;
-  const size_t smem = tile * ((p.reqLog ? 1 : 0) + q.stageMag);
+  const size_t smem = (q.stageMag ? tile : 0) + (p.reqLog ? (size_t)p.nSrc * p.F * sizeof(float) : 0);
+  if (staged) *staged = q.stageMag;
+  if (smemBytes) *smemBytes = (int)smem;
   cudaError_t e = cudaFuncSetAttribute(spectral_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   spectral_kernel<<<p.nTiles, kSpecThreads, smem, st>>>(q);

@@ -13,6 +13,7 @@ import numpy as np
 from . import capi
 
 LldLaunch = namedtuple("LldLaunch", "kernel grid n_chunks")
+RunInfo = namedtuple("RunInfo", "pieces spectral_staged spectral_smem")
 
 
 def _comp(ctype, name, reader, writer, **fields):
@@ -241,6 +242,14 @@ class Plan:
         if self._L.osm_b200_plan_last_lld_launch(self._h, C.byref(nm), C.byref(grid), C.byref(n_chunks)) != capi.OK:
             raise RuntimeError(capi.last_error())
         return LldLaunch(nm.value.decode() if nm.value else None, grid.value, n_chunks.value)
+
+    def last_run_info(self):
+        """(pipeline pieces of run_host, spectral_kernel staging path -- 1 staged, 0 global, -1 none -- and its shared memory in
+        bytes) of the last run"""
+        a, b, c = C.c_int32(0), C.c_int32(0), C.c_int32(0)
+        if self._L.osm_b200_plan_last_run_info(self._h, C.byref(a), C.byref(b), C.byref(c)) != capi.OK:
+            raise RuntimeError(capi.last_error())
+        return RunInfo(a.value, b.value, c.value)
 
     def set_profiling(self, on):
         """per-kernel CUDA-event timing of run_device (serialises the step on one stream)"""

@@ -75,7 +75,7 @@ class PitchAcf(C.Structure):
                 ("acfCepsNormOutput", C.c_int), ("maxPitch", C.c_double),
                 ("voiceProb", C.c_int), ("voiceQual", C.c_int), ("HNR", C.c_int), ("HNRdB", C.c_int),
                 ("linHNR", C.c_int), ("F0", C.c_int), ("F0raw", C.c_int), ("F0env", C.c_int),
-                ("voicingCutoff", C.c_double)]
+                ("voicingCutoff", C.c_double), ("oldCompatCepstrum", C.c_int)]
 
 
 def pitchacf_cfg(**kw):
@@ -100,6 +100,22 @@ def pitchacf(pcm, fe, cfg, n_chan=1, taps=False):
     r = L.osm_or_pitchacf(C.byref(fe), C.byref(cfg), pcm.ctypes.data_as(C.POINTER(C.c_int16)), C.c_long(nS),
                           C.c_int(n_chan), _fp(out), _fp(ta), _fp(tc))
     assert r == max(T, 0)
+    return (out, ta, tc) if taps else out
+
+
+def pitchacf_from_mag(mag, fe, cfg, taps=False):
+    """cAcf x2 -> cPitchACF on given magnitudes [T, nfft/2+1] of one utterance (fe gives the FFT size and frame length)"""
+    mag = np.ascontiguousarray(mag, np.float32)
+    T = mag.shape[0]
+    L = lib()
+    L.osm_or_pitchacf_from_mag.restype = C.c_long
+    K = L.osm_or_pitchacf_num_out(C.byref(cfg))
+    out = np.zeros((T, K), np.float32)
+    n = mag.shape[1] - 1
+    ta = np.zeros((T, n), np.float32) if taps else None
+    tc = np.zeros((T, n), np.float32) if taps else None
+    r = L.osm_or_pitchacf_from_mag(C.byref(fe), C.byref(cfg), _fp(mag), C.c_long(T), _fp(out), _fp(ta), _fp(tc))
+    assert r == T, (r, T)
     return (out, ta, tc) if taps else out
 
 
@@ -158,6 +174,18 @@ def _run_static(fn_name, nout_name, fe, cfg, pcm, n_chan, extra=()):
 
 def spectral(pcm, fe, cfg, n_chan=1):
     return _run_static("osm_or_spectral", "osm_or_spectral_num_out", fe, cfg, pcm, n_chan)
+
+
+def spectral_from_mag(mag, fe, cfg):
+    """cSpectral on given magnitudes [T, nfft/2+1] of one utterance (fe gives the bin frequencies)"""
+    mag = np.ascontiguousarray(mag, np.float32)
+    T = mag.shape[0]
+    L = lib()
+    L.osm_or_spectral_from_mag.restype = C.c_long
+    out = np.zeros((T, L.osm_or_spectral_num_out(C.byref(cfg))), np.float32)
+    r = L.osm_or_spectral_from_mag(C.byref(fe), C.byref(cfg), _fp(mag), C.c_long(T), _fp(out))
+    assert r == T, (r, T)
+    return out
 
 
 def energy(pcm, fe, cfg=None, windowed=0, n_chan=1):

@@ -1393,39 +1393,60 @@ static void spec_mag_frame(void *vctx, const float *mag, long nb, float *dst)
   spectral_frame((spec_ctx *)vctx, mag, dst);
 }
 
+/* cSpectral's per-frame context for the geometry of fe (bin frequencies, spectral range, sharpness weights) */
+static void spec_ctx_init(spec_ctx *c, const osm_or_frontend *fe, const osm_or_spectral_cfg *sp)
+{
+  long N = osm_or_frame_size_samples(fe);
+  long nfft = osm_or_fft_size(N), Nsrc = nfft / 2 + 1;
+  memset(c, 0, sizeof *c);
+  c->sp = sp; c->Nsrc = Nsrc; c->fsSec = osm_or_fft_frame_size_sec(fe);
+  c->frq = (double *)malloc(sizeof(double) * Nsrc);
+  double F0 = (double)(1.0) / (double)c->fsSec;                /* transformFft.cpp:111-115 */
+  for (long i = 0; i < Nsrc; i++) c->frq[i] = F0 * (double)i;
+  /* spectral range :625-647 */
+  long lo = (long)sp->freqRangeLo, hi = (long)sp->freqRangeHi;
+  if (lo == hi && hi == 0) { c->loBin = 1; c->hiBin = Nsrc - 1; }
+  else {
+    c->loBin = -1; c->hiBin = -1;
+    for (long i = 0; i < Nsrc; i++) {
+      if ((double)lo >= c->frq[i]) c->loBin = i;
+      if ((double)hi > c->frq[i]) c->hiBin = i;
+    }
+    if (c->hiBin == -1 || c->hiBin >= Nsrc) c->hiBin = Nsrc - 1;
+    if (c->loBin < 0) c->loBin = 0;
+  }
+  c->prev = (float *)calloc(Nsrc, sizeof(float));
+  c->sharpW = (double *)calloc(Nsrc, sizeof(double));
+  for (long j = c->loBin; j <= c->hiBin; j++) {                /* :1443-1453 (linear scale -> bark) */
+    double fb = bark_fwd(c->frq[j]);
+    c->sharpW[j - c->loBin] = fb * sharp_g(fb);
+  }
+}
+
+static void spec_ctx_free(spec_ctx *c) { free(c->frq); free(c->prev); free(c->sharpW); }
+
 long osm_or_spectral(const osm_or_frontend *fe, const osm_or_spectral_cfg *sp,
                      const int16_t *pcm, long L, int n_chan, float *out)
 {
   long N = osm_or_frame_size_samples(fe), H = osm_or_frame_step_samples(fe);
-  long nfft = osm_or_fft_size(N), Nsrc = nfft / 2 + 1;
   long T = osm_or_num_frames(L, N, H);
   if (T <= 0) return 0;
-  spec_ctx c; memset(&c, 0, sizeof c);
-  c.sp = sp; c.Nsrc = Nsrc; c.fsSec = osm_or_fft_frame_size_sec(fe);
-  c.frq = (double *)malloc(sizeof(double) * Nsrc);
-  double F0 = (double)(1.0) / (double)c.fsSec;                 /* transformFft.cpp:111-115 */
-  for (long i = 0; i < Nsrc; i++) c.frq[i] = F0 * (double)i;
-  /* spectral range :625-647 */
-  long lo = (long)sp->freqRangeLo, hi = (long)sp->freqRangeHi;
-  if (lo == hi && hi == 0) { c.loBin = 1; c.hiBin = Nsrc - 1; }
-  else {
-    c.loBin = -1; c.hiBin = -1;
-    for (long i = 0; i < Nsrc; i++) {
-      if ((double)lo >= c.frq[i]) c.loBin = i;
-      if ((double)hi > c.frq[i]) c.hiBin = i;
-    }
-    if (c.hiBin == -1 || c.hiBin >= Nsrc) c.hiBin = Nsrc - 1;
-    if (c.loBin < 0) c.loBin = 0;
-  }
-  c.prev = (float *)calloc(Nsrc, sizeof(float));
-  c.sharpW = (double *)calloc(Nsrc, sizeof(double));
-  for (long j = c.loBin; j <= c.hiBin; j++) {                  /* :1443-1453 (linear scale -> bark) */
-    double fb = bark_fwd(c.frq[j]);
-    c.sharpW[j - c.loBin] = fb * sharp_g(fb);
-  }
+  spec_ctx c;
+  spec_ctx_init(&c, fe, sp);
   int K = osm_or_spectral_num_out(sp);
   run_frames(fe, pcm, L, n_chan, spec_mag_frame, &c, K, out, NULL);
-  free(c.frq); free(c.prev); free(c.sharpW);
+  spec_ctx_free(&c);
+  return T;
+}
+
+long osm_or_spectral_from_mag(const osm_or_frontend *fe, const osm_or_spectral_cfg *sp, const float *mag, long T, float *out)
+{
+  if (T <= 0) return 0;
+  spec_ctx c;
+  spec_ctx_init(&c, fe, sp);
+  int K = osm_or_spectral_num_out(sp);
+  for (long t = 0; t < T; t++) spectral_frame(&c, mag + t * c.Nsrc, out + t * K);
+  spec_ctx_free(&c);
   return T;
 }
 
@@ -1442,7 +1463,7 @@ typedef struct {
   const osm_or_pitchacf_cfg *pc;
   long Nsrc, N;             /* magnitude bins, FFT size */
   double *costab;           /* cos(2 pi i / N) */
-  float *acf, *cep;         /* N/2 each */
+  float *acf, *cep;         /* N/2 each, adjacent: acf is the reader's concatenated [acf ; cepstrum] */
   float fsSec;              /* (float) frameSizeSec of the acf level (pitchACF.cpp:107-110) */
   float lastPitch, lastlastPitch, glMeanPitch, pitchEnv;
   int onsFlag;
@@ -1456,17 +1477,19 @@ static void acf_level(const pacf_ctx *c, const float *src, int usePower, int cep
 {
   long Nsrc = c->Nsrc, N = c->N, Ndst = Nsrc - 1;    /* symmetricData=1: nOutEl = nEl - 1 (acf.cpp:123-128) */
   float *r = (float *)malloc(sizeof(float) * Nsrc);
+  const int oldCompat = cepstrum && c->pc->oldCompatCepstrum;
   for (long k = 0; k < Nsrc; k++) {
     float v = usePower ? src[k] * src[k] : src[k];    /* :253-261 */
-    if (cepstrum) v = (v > 0.0) ? (float)log(v + 1.0) : 0.0f;   /* :289-305 */
+    if (oldCompat) { if (k > 0 && k < Nsrc - 1) v = (v > 0.0) ? logf(v) : 0.0f; }   /* :276-286: float log, DC / Nyquist as is */
+    else if (cepstrum) v = (v > 0.0) ? (float)log(v + 1.0) : 0.0f;   /* :289-305 */
     r[k] = v;
   }
   for (long j = 0; j < Ndst; j++) {
     double x = ((double)r[0] + (double)r[N / 2] * ((j & 1) ? -1.0 : 1.0)) / 2.0;
     for (long k = 1; k < N / 2; k++) x += (double)r[k] * c->costab[(j * k) % N];
     float d = (float)x;
-    if (c->pc->acfCepsNormOutput) d = d / (float)Nsrc;  /* :321-325 */
-    if (cepstrum) { if (absCeps) d = fabsf(d); }         /* :327-341 */
+    if (c->pc->acfCepsNormOutput && !oldCompat) d = d / (float)Nsrc;  /* :321-325 (oldCompatCepstrum: acf.cpp:104) */
+    if (cepstrum) { if (absCeps || oldCompat) d = fabsf(d); }         /* :327-341 (oldCompatCepstrum: acf.cpp:105) */
     else d = fabsf(d);                                   /* :342-344 */
     dst[j] = d;
   }
@@ -1590,23 +1613,49 @@ static void pitchacf_frame(void *vctx, const float *mag, long nb, float *dst)
   }
 }
 
+/* preskip (pitchACF.cpp:155-159) of fe's geometry; the reference reads [acf ; cepstrum][preskip], outside its input from
+ * preskip = nfft on: refused (-1) like the plan refuses it */
+static int pacf_ctx_init(pacf_ctx *c, const osm_or_frontend *fe, const osm_or_pitchacf_cfg *pc)
+{
+  long N0 = osm_or_frame_size_samples(fe);
+  long nfft = osm_or_fft_size(N0), Nsrc = nfft / 2 + 1;
+  memset(c, 0, sizeof *c);
+  c->pc = pc; c->Nsrc = Nsrc; c->N = nfft;
+  c->fsSec = (float)osm_or_fft_frame_size_sec(fe);     /* cAcf keeps the level's frameSizeSec */
+  double maxPitch = pc->maxPitch < 0.0 ? 0.0 : pc->maxPitch;
+  int preskip = (maxPitch <= 0.0) ? 0 : (int)(1.0 / (maxPitch * ((double)c->fsSec / (double)nfft)));
+  if (preskip >= nfft) return -1;
+  c->costab = (double *)malloc(sizeof(double) * nfft);
+  for (long i = 0; i < nfft; i++) c->costab[i] = cos(2.0 * M_PI * (double)i / (double)nfft);
+  c->acf = (float *)malloc(sizeof(float) * 2 * (Nsrc - 1));
+  c->cep = c->acf + (Nsrc - 1);
+  return 0;
+}
+
 long osm_or_pitchacf(const osm_or_frontend *fe, const osm_or_pitchacf_cfg *pc,
                      const int16_t *pcm, long L, int n_chan, float *out, float *tap_acf, float *tap_cep)
 {
   long N0 = osm_or_frame_size_samples(fe), H = osm_or_frame_step_samples(fe);
-  long nfft = osm_or_fft_size(N0), Nsrc = nfft / 2 + 1;
   long T = osm_or_num_frames(L, N0, H);
   if (T <= 0) return 0;
-  pacf_ctx c; memset(&c, 0, sizeof c);
-  c.pc = pc; c.Nsrc = Nsrc; c.N = nfft;
-  c.costab = (double *)malloc(sizeof(double) * nfft);
-  for (long i = 0; i < nfft; i++) c.costab[i] = cos(2.0 * M_PI * (double)i / (double)nfft);
-  c.acf = (float *)malloc(sizeof(float) * Nsrc);
-  c.cep = (float *)malloc(sizeof(float) * Nsrc);
-  c.fsSec = (float)osm_or_fft_frame_size_sec(fe);      /* cAcf keeps the level's frameSizeSec */
+  pacf_ctx c;
+  if (pacf_ctx_init(&c, fe, pc) != 0) return -1;
   c.tap_acf = tap_acf; c.tap_cep = tap_cep;
   int K = osm_or_pitchacf_num_out(pc);
   run_frames(fe, pcm, L, n_chan, pitchacf_frame, &c, K, out, NULL);
-  free(c.costab); free(c.acf); free(c.cep);
+  free(c.costab); free(c.acf);
+  return T;
+}
+
+long osm_or_pitchacf_from_mag(const osm_or_frontend *fe, const osm_or_pitchacf_cfg *pc, const float *mag, long T, float *out,
+                              float *tap_acf, float *tap_cep)
+{
+  if (T <= 0) return 0;
+  pacf_ctx c;
+  if (pacf_ctx_init(&c, fe, pc) != 0) return -1;
+  c.tap_acf = tap_acf; c.tap_cep = tap_cep;
+  int K = osm_or_pitchacf_num_out(pc);
+  for (long t = 0; t < T; t++) pitchacf_frame(&c, mag + t * c.Nsrc, c.Nsrc, out + t * K);
+  free(c.costab); free(c.acf);
   return T;
 }

@@ -103,6 +103,8 @@ typedef struct {            /* cAcf x2 + cPitchACF (dspcore/acf.cpp, lldcore/pit
   double maxPitch;          /* 500 */
   int voiceProb, voiceQual, HNR, HNRdB, linHNR, F0, F0raw, F0env;
   double voicingCutoff;     /* 0.55 */
+  int oldCompatCepstrum;    /* [cep] oldCompatCepstrum (0): log(x) without +1, DC / Nyquist un-logged; forces absCepstrum = 1
+                               and acfCepsNormOutput = 0 on the cepstrum (dspcore/acf.cpp:103-109,276-286) */
 } osm_or_pitchacf_cfg;
 
 /* ---- geometry (integer work, must be bit exact) ---- */
@@ -148,6 +150,9 @@ void osm_or_ll1(const float *x, long T, int K, float *out);
 int  osm_or_spectral_num_out(const osm_or_spectral_cfg *sp);
 long osm_or_spectral(const osm_or_frontend *fe, const osm_or_spectral_cfg *sp,
                      const int16_t *pcm, long n_samples, int n_chan, float *out);
+/* the same on given magnitudes: mag = [T][nfft/2+1] (the FFT size and bin frequencies of fe's geometry) -> out = [T][num_out];
+ * osm_or_spectral is the oracle's own FFT front end followed by this */
+long osm_or_spectral_from_mag(const osm_or_frontend *fe, const osm_or_spectral_cfg *sp, const float *mag, long T, float *out);
 int  osm_or_energy_num_out(const osm_or_energy_cfg *en);
 long osm_or_energy(const osm_or_frontend *fe, const osm_or_energy_cfg *en, int windowed,
                    const int16_t *pcm, long n_samples, int n_chan, float *out);
@@ -157,6 +162,9 @@ int  osm_or_pitchacf_num_out(const osm_or_pitchacf_cfg *pc);
 long osm_or_pitchacf(const osm_or_frontend *fe, const osm_or_pitchacf_cfg *pc,
                      const int16_t *pcm, long n_samples, int n_chan, float *out,
                      float *tap_acf, float *tap_cep);
+/* the same on given magnitudes [T][nfft/2+1] of one utterance (the smoothing state starts at its frame 0) */
+long osm_or_pitchacf_from_mag(const osm_or_frontend *fe, const osm_or_pitchacf_cfg *pc, const float *mag, long T, float *out,
+                              float *tap_acf, float *tap_cep);
 int  osm_or_mzcr_num_out(const osm_or_mzcr_cfg *mz);
 int  osm_or_intensity_num_out(const osm_or_intensity_cfg *in);
 /* cIntensity on the framer level: out = [T][num_out] (lldcore/intensity.cpp:86-146) */
