@@ -15,6 +15,8 @@
 //           (functionalRegression.cpp:263-290), which need the results of pass 1
 // then a warp-wide bitonic sort of the shared copy for cFunctionalPercentiles (the reference sorts with std::sort,
 // functionals.cpp:296-299), and lane 0 assembles the values in the reference's order.
+// Contours longer than kMaxShort rows (long_contours.hpp) run the same statements with the copy in a work space slice in HBM, and
+// their percentiles come from a radix rank selection (pctl_select_kernel, rank_select.cuh) instead of a sort.
 // All accumulators are double like the reference's; the reference adds sequentially, a warp adds 32 strided partial sums and
 // combines them by shuffles -- a reordering of double additions, 1e-16 relative, invisible in the float results.
 // Compiled with -fmad=false (the float expressions of the percentile interpolation keep their two roundings).
@@ -30,14 +32,16 @@
 #include "../../include/osm_b200_functionals.h"
 #include "cuda_owned.hpp"
 #include "functionals_seq.cuh"
+#include "long_contours.hpp"
 #include "plan.hpp"
+#include "rank_select.cuh"
 
 namespace osm {
 namespace {
 
 constexpr int kFnWarps = 4;
 constexpr int kFnThreads = kFnWarps * 32;
-constexpr int kMaxSort = 8192;              // longest filtered contour with percentiles enabled (32 KB per warp)
+constexpr int kSelThreads = 512;
 
 struct FnParams {
   const float *rows; int rowStride; int nIn;
@@ -54,6 +58,8 @@ struct FnParams {
   osm_b200_functionals_spec s;
   int extNorm, meanNorm;                    // resolved time normalisations
   int needReg, enQreg;
+  LongContour *lc; int nLong;               // long path: this chunk's contours, one slice of wsStride floats each in ws
+  float *ws; long long wsStride;
 };
 
 __device__ __forceinline__ double wsum(double v)
@@ -94,18 +100,27 @@ __device__ float index_pctl(double p, const float *s, long long N)          // g
   return s[r];
 }
 
+// kLong = false: one warp per (utterance, element) of the grid, the contour copy in shared memory (contours of at most kMaxShort
+// rows).  kLong = true: one warp per contour of p.lc, the copy in that contour's work space slice in global memory (sortCap /
+// listOff / lensOff describe the chunk's slice); the percentiles are left to pctl_select_kernel, which reads the same copy.  The
+// statements are the same in both.
+template <bool kLong>
 __global__ void __launch_bounds__(kFnThreads) functionals_kernel(const FnParams p)
 {
   extern __shared__ float fnSort[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nW = blockDim.x >> 5;                                   // 1 .. kFnWarps: fewer when long contours need the shared memory
   const int groups = (p.nIn + nW - 1) / nW;
-  const int u = blockIdx.x / groups, e = (blockIdx.x % groups) * nW + warp;
+  const int c = blockIdx.x * nW + warp;                             // long path: this warp's contour
+  if (kLong && c >= p.nLong) return;
+  const int u = kLong ? p.lc[c].u : blockIdx.x / groups, e = kLong ? p.lc[c].e : (blockIdx.x % groups) * nW + warp;
   if (e >= p.nIn) return;
   const long long T = p.nRows[u];
   const float *col = p.rows + p.rowOff[u] * (long long)p.rowStride + (p.cols ? p.cols[e] : e);
   float *out = p.out + (long long)u * p.outStride + (long long)e * p.nVals;
-  float *sbuf = fnSort + (size_t)warp * p.perWarp;
+  // the long path's slice: segment lengths / lag buffer | contour copy | extrema list, so that lensOff = -lensFloats and every
+  // offset from sbuf stays below 2^31 floats
+  float *sbuf = kLong ? p.ws + (long long)c * p.wsStride - p.lensOff : fnSort + (size_t)warp * p.perWarp;
   const Keep keep{p.s.nonZeroFuncts};
   const unsigned ltMask = (1u << lane) - 1u;
 
@@ -138,6 +153,7 @@ __global__ void __launch_bounds__(kFnThreads) functionals_kernel(const FnParams 
     cnt += __popc(m);
   }
   const long long N = cnt;                 // uniform
+  if (kLong && lane == 0) p.lc[c].n = (int)N;
   if (N == 0) {                            // every sub-component returns nothing: zero fill (functionals.cpp:316-320)
     for (int v = lane; v < p.nVals; v += 32) out[v] = 0.0f;
     return;
@@ -195,7 +211,7 @@ __global__ void __launch_bounds__(kFnThreads) functionals_kernel(const FnParams 
     }
   }
 
-  // ---------------- order-dependent functionals on the shared copy of the filtered contour ----------------
+  // ---------------- order-dependent functionals on the copy of the filtered contour ----------------
   __syncwarp();
   for (int fi = 0; fi < p.s.n_enabled; fi++) {
     float *o = out + p.valOff[fi];
@@ -330,7 +346,7 @@ __global__ void __launch_bounds__(kFnThreads) functionals_kernel(const FnParams 
   // ---------------- sorted copy for the percentiles ----------------
   bool needSort = false;
   for (int i = 0; i < p.s.n_enabled; i++) needSort = needSort || p.s.enabled[i] == OSM_B200_F_PERCENTILES;
-  if (needSort) {
+  if (!kLong && needSort) {
     int n2 = 32;
     while (n2 < N) n2 <<= 1;
     __syncwarp();
@@ -418,6 +434,7 @@ __global__ void __launch_bounds__(kFnThreads) functionals_kernel(const FnParams 
         }
       } break;
       case OSM_B200_F_PERCENTILES: {
+        if (kLong) break;                                              // pctl_select_kernel
         const auto &P = p.s.percentiles;
         const float q1 = P.interp ? interp_pctl(0.25, sbuf, N) : index_pctl(0.25, sbuf, N);
         const float q2 = P.interp ? interp_pctl(0.50, sbuf, N) : index_pctl(0.50, sbuf, N);
@@ -458,6 +475,52 @@ __global__ void __launch_bounds__(kFnThreads) functionals_kernel(const FnParams 
         if (R.centroid) out[n++] = (float)fin(centroid);
       } break;
     }
+  }
+}
+
+// cFunctionalPercentiles of the long path: one CTA per contour of the chunk finds every rank the percentile block reads in one
+// MSB-first radix walk over the contour's copy (rank_select.cuh) and writes the block.  Walkers whose prefixes agree share a histogram.
+struct SelParams {
+  const LongContour *lc; const float *ws; long long wsStride; int copyOff;
+  float *out; long long outStride; int nVals, valOff;
+  decltype(osm_b200_functionals_spec::percentiles) P;
+};
+
+__global__ void __launch_bounds__(kSelThreads) pctl_select_kernel(const __grid_constant__ SelParams p)
+{
+  __shared__ unsigned hist[rsel::kMaxRanks][rsel::kDigits];
+  __shared__ long long rank[rsel::kMaxRanks], rem[rsel::kMaxRanks];
+  __shared__ uint32_t pre[rsel::kMaxRanks];
+  __shared__ int lead[rsel::kMaxRanks];
+  const LongContour &d = p.lc[blockIdx.x];
+  const long long N = d.n;
+  if (N == 0) return;                                                // functionals_kernel wrote the zero fill
+  const float *x = p.ws + (long long)blockIdx.x * p.wsStride + p.copyOff;
+  const int t = threadIdx.x, nr = 2 * (3 + p.P.n_percentile);
+  if (t == 0) rsel::pctl_walkers(p.P, N, rank);
+  __syncthreads();
+  if (t < nr) { rem[t] = rank[t]; pre[t] = 0; }
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    __syncthreads();
+    if (t < nr) { int l = 0; while (pre[l] != pre[t]) l++; lead[t] = l; }
+    for (int i = t; i < nr * rsel::kDigits; i += blockDim.x) hist[i / rsel::kDigits][i % rsel::kDigits] = 0u;
+    __syncthreads();
+    for (long long i = t; i < N; i += blockDim.x) {
+      const uint32_t k = rsel::key(x[i]), hi = rsel::prefix(k, shift);
+      for (int w = 0; w < nr; w++)
+        if (lead[w] == w && pre[w] == hi) { atomicAdd(&hist[w][rsel::digit(k, shift)], 1u); break; }
+    }
+    __syncthreads();
+    uint32_t next = 0;
+    if (t < nr) { long long r = rem[t]; next = (pre[t] << 8) | (uint32_t)rsel::digit_of_rank(hist[lead[t]], r); rem[t] = r; }
+    __syncthreads();
+    if (t < nr) pre[t] = next;
+  }
+  __syncthreads();
+  if (t == 0) {
+    float sel[rsel::kMaxRanks];
+    for (int w = 0; w < nr; w++) sel[w] = rsel::value(pre[w]);
+    rsel::pctl_block(p.P, N, rank, sel, p.out + (long long)d.u * p.outStride + (long long)d.e * p.nVals + p.valOff);
   }
 }
 
@@ -508,6 +571,8 @@ struct osm_b200_functionals {
   DevBuf<long long> dMeta;
   DevBuf<float> dIn, dOut;                     // run_host staging: one float more than the largest batch so far
   DevBuf<int> dCols; std::vector<int> hCols;
+  DevBuf<float> dWs;                           // long contours: work space, at most kLongWsCapFloats unless one contour needs more
+  DevBuf<LongContour> dLong; std::vector<LongContour> longs; std::vector<LongChunk> chunks;
 
   ~osm_b200_functionals() { if (device >= 0) cudaSetDevice(device); }
 };
@@ -755,16 +820,23 @@ osm_b200_status osm_b200_functionals_run_device_cols(osm_b200_functionals *f, co
       CU(cudaMemcpy(f->dCols.p, f->hCols.data(), sizeof(int) * (size_t)f->nIn, cudaMemcpyHostToDevice));
     }
   }
+  // meta: row offsets | row counts of the shared-memory launch (0 for a long contour: that launch zero-fills its row, the long path
+  // overwrites it later on the stream) | row counts
+  const bool needCopy = f->hasPct || f->hasSeq;
   long long maxT = 0;
-  std::vector<long long> meta(2 * (size_t)n_utt);
+  int nLongUtt = 0;
+  std::vector<long long> meta(3 * (size_t)n_utt);
   for (int u = 0; u < n_utt; u++) {
     if (n_rows[u] < 0 || row_offsets[u] < 0) return set_last_error(OSM_B200_ERR_INVALID, "negative row offset / count");
-    meta[u] = row_offsets[u]; meta[n_utt + u] = n_rows[u];
-    maxT = std::max<long long>(maxT, n_rows[u]);
+    if (needCopy && n_rows[u] >= kMaxLongRows)
+      return set_last_error(OSM_B200_ERR_UNSUPPORTED, "cFunctionals (Percentiles, Times, Lpc, Segments, Peaks2): contours of 2^30 = 1073741824 frames or more are not supported (Peaks2 packs a frame index and a type bit into 32 bits)");
+    const bool isLong = needCopy && n_rows[u] > kMaxShort;
+    nLongUtt += isLong;
+    meta[u] = row_offsets[u]; meta[n_utt + u] = isLong ? 0 : n_rows[u]; meta[2 * (size_t)n_utt + u] = n_rows[u];
+    maxT = std::max<long long>(maxT, meta[n_utt + u]);
   }
   int sortCap = 0;
-  if (f->hasPct || f->hasSeq) {
-    if (maxT > kMaxSort) return set_last_error(OSM_B200_ERR_UNSUPPORTED, "cFunctionals (Percentiles, Times, Lpc, Segments, Peaks2): contours longer than 8192 frames are not supported");
+  if (needCopy) {
     sortCap = 32;
     while (sortCap < maxT) sortCap <<= 1;
   }
@@ -777,6 +849,12 @@ osm_b200_status osm_b200_functionals_run_device_cols(osm_b200_functionals *f, co
   if ((size_t)nWarps * perWarp * sizeof(float) > 200 * 1024) return set_last_error(OSM_B200_ERR_UNSUPPORTED, "cFunctionals: contour too long for the shared-memory work space");
   CU(f->dMeta.reserve_exact(meta.size()));
   CU(cudaMemcpyAsync(f->dMeta.p, meta.data(), meta.size() * sizeof(long long), cudaMemcpyHostToDevice, st));
+  if (nLongUtt > 0) {
+    const long long wsFloats = plan_long_contours(n_rows, n_utt, f->nIn, f->hasPeaks ? 2 : 0, lensFloats, kLongWsCapFloats, f->longs, f->chunks);
+    CU(f->dWs.reserve_exact((size_t)wsFloats));
+    CU(f->dLong.reserve_exact(f->longs.size()));
+    CU(cudaMemcpyAsync(f->dLong.p, f->longs.data(), f->longs.size() * sizeof(LongContour), cudaMemcpyHostToDevice, st));
+  }
   CU(cudaStreamSynchronize(st));                  // `meta` is a local: the copy must have left the host buffer
   FnParams p;
   memset(&p, 0, sizeof p);
@@ -795,11 +873,34 @@ osm_b200_status osm_b200_functionals_run_device_cols(osm_b200_functionals *f, co
   const auto &R = f->spec.regression;
   for (int i = 0; i < f->spec.n_enabled; i++) p.needReg = p.needReg || f->spec.enabled[i] == OSM_B200_F_REGRESSION;
   p.enQreg = R.qregc1 || R.qregc2 || R.qregc3 || R.qregerrA || R.qregerrQ || R.centroid;     // functionalRegression.cpp:108-117
-  const size_t smem = (size_t)nWarps * perWarp * sizeof(float);
-  if (smem > 48 * 1024) CU(cudaFuncSetAttribute(functionals_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int groups = (f->nIn + nWarps - 1) / nWarps;
-  functionals_kernel<<<(unsigned)((long long)n_utt * groups), nWarps * 32, smem, st>>>(p);
-  CU(cudaGetLastError());
+  if (nLongUtt < n_utt) {
+    const size_t smem = (size_t)nWarps * perWarp * sizeof(float);
+    if (smem > 48 * 1024) CU(cudaFuncSetAttribute(functionals_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const int groups = (f->nIn + nWarps - 1) / nWarps;
+    functionals_kernel<false><<<(unsigned)((long long)n_utt * groups), nWarps * 32, smem, st>>>(p);
+    CU(cudaGetLastError());
+  }
+  if (nLongUtt == 0) return OSM_B200_OK;
+  // long contours, chunk by chunk through the one work space: a warp per contour (one per CTA, so that a chunk spreads over the
+  // SMs), then a CTA per contour for the percentiles
+  p.nRows = f->dMeta.p + 2 * (size_t)n_utt;
+  p.ws = f->dWs.p;
+  SelParams sp;
+  memset(&sp, 0, sizeof sp);
+  sp.ws = f->dWs.p; sp.copyOff = lensFloats; sp.out = d_out; sp.outStride = out_stride; sp.nVals = f->nVals; sp.P = f->spec.percentiles;
+  for (int i = 0; i < f->spec.n_enabled; i++) if (f->spec.enabled[i] == OSM_B200_F_PERCENTILES) sp.valOff = p.valOff[i];
+  for (const LongChunk &ch : f->chunks) {
+    const int nC = ch.end - ch.begin;
+    p.lc = f->dLong.p + ch.begin; p.nLong = nC;
+    p.sortCap = ch.cap; p.listOff = ch.cap; p.lensOff = -lensFloats; p.wsStride = long_slice_floats(ch.cap, f->hasPeaks ? 2 : 0, lensFloats);
+    functionals_kernel<true><<<(unsigned)nC, 32, 0, st>>>(p);
+    CU(cudaGetLastError());
+    if (f->hasPct) {
+      sp.lc = p.lc; sp.wsStride = p.wsStride;
+      pctl_select_kernel<<<(unsigned)nC, kSelThreads, 0, st>>>(sp);
+      CU(cudaGetLastError());
+    }
+  }
   return OSM_B200_OK;
 }
 
